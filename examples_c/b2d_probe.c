@@ -35,7 +35,7 @@ int main(int argc, char** argv) {
   b2d_ctx* ctx = NULL;
   int rc = b2d_ctx_create_fn(0, 1, 0, (size_t)1 << 20, 0u, &ctx);
   if (rc != B2D_OK) {
-    printf("b2d_ctx_create -> %d (%s): no usable B200 here, which is the documented error path\n", rc, b2d_last_error_fn(NULL));
+    printf("b2d_ctx_create -> %d (%s): no usable H100 here, which is the documented error path\n", rc, b2d_last_error_fn(NULL));
     return 0;
   }
   int algo = 0, grid = 0, block = 0;

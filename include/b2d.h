@@ -1,8 +1,8 @@
 /*
- * b2d.h — C ABI of libb2d: the B200-native DDP gradient-sync data path.
+ * b2d.h — C ABI of libb2d: the H100-native (sm_90a) DDP gradient-sync data path.
  *
  * This is the drop-in boundary of the repo (DESIGN.md §2, SURVEY.md §8b).  The
- * library replaces, for one 8xB200 NVSwitch box, the collectives that the
+ * library replaces, for one 8xH100 NVSwitch box, the collectives that the
  * reference's strategies reach through torch DDP / FairScale:
  *
  *   reference seam                                   replaced by
@@ -49,8 +49,8 @@ extern "C" {
 #endif
 
 #define B2D_VERSION 110          /* 0.1.10 */
-#define B2D_MAX_WORLD 8          /* one NVSwitch domain: 8 x B200 */
-#define B2D_MAX_BLOCKS 296       /* 2 x 148 SMs */
+#define B2D_MAX_WORLD 8          /* one NVSwitch domain: 8 x H100 */
+#define B2D_MAX_BLOCKS 264       /* 2 x 132 SMs (H100 SXM) */
 #define B2D_HANDLE_BYTES 256     /* size of the blob b2d_ctx_export() writes */
 
 typedef struct b2d_ctx b2d_ctx;

@@ -1,4 +1,4 @@
-"""ray_lightning_b200 — a B200-native DDP gradient-sync path behind ray_lightning's plugin API.
+"""ray_lightning_b200 — an H100-native (sm_90a) DDP gradient-sync path behind ray_lightning's plugin API.
 
 Public surface == the reference's (ray_lightning/__init__.py:1-5)."""
 from .ray_ddp import RayStrategy

@@ -12,7 +12,7 @@ _LIB_LOCK = threading.Lock()
 
 HANDLE_BYTES = 256
 MAX_WORLD = 8
-MAX_BLOCKS = 296
+MAX_BLOCKS = 264
 
 WIRE_FP32, WIRE_BF16 = 0, 1
 ALGO_AUTO, ALGO_ONE_SHOT, ALGO_TWO_SHOT, ALGO_NVLS, ALGO_TWO_SHOT_TMA, ALGO_STAGED, ALGO_NVLS_FUSED = 0, 1, 2, 3, 4, 5, 6
@@ -41,7 +41,7 @@ RTO_ZERO_GRADS, RTO_ACCUMULATE, RTO_NVLS = 1, 2, 4
 
 
 class B2DUnavailableError(RuntimeError):
-    """libb2d.so is missing and could not be built: the B200 data path cannot run."""
+    """libb2d.so is missing and could not be built: the GPU data path cannot run."""
 
 
 class B2DError(RuntimeError):
@@ -158,7 +158,7 @@ def load(build_if_missing=True):
         if not os.path.exists(path):
             raise B2DUnavailableError(
                 "libb2d.so not found at %s; run `python -m ray_lightning_b200.csrc.build` "
-                "(there is no CPU fallback for the B200 gradient-sync path)" % path)
+                "(there is no CPU fallback for the GPU gradient-sync path)" % path)
         try:
             lib = ctypes.CDLL(path)
         except OSError as e:

@@ -1,4 +1,4 @@
-"""Tensor-level host side of the B200 gradient-sync path.
+"""Tensor-level host side of the H100 gradient-sync path.
 
 * ``Communicator``   — one rank of a one-process-per-GPU job (the Ray-actor model of
   ray_lightning/launchers/ray_launcher.py:105-114): creates the libb2d context, exchanges the
@@ -234,7 +234,7 @@ class Communicator(_Base):
                  nvls="auto", timeout_ms=None, max_ctas=None, one_shot_max_bytes=None, chunk_bytes=None,
                  exch_ctas=None):
         if not torch.cuda.is_available():
-            raise _b2d.B2DUnavailableError("CUDA is not available: the B200 gradient-sync path has no CPU fallback")
+            raise _b2d.B2DUnavailableError("CUDA is not available: the H100 gradient-sync path has no CPU fallback")
         self.rank, self.world, self.device_index = rank, world, device_index
         self.group = group
         self.mem = mem

@@ -229,9 +229,8 @@ struct b2d_ctx {
   unsigned long long* trace_dev = nullptr;   // debug: per-block phase stamps of the LAST allreduce launch
   int trace_grid = 0;
 
-  // 64 CTAs: measured inside a ResNet-50 step on 8 GPUs a 128-CTA grid waits longer for SMs to drain from
-  // the backward kernels than it gains (avg launch 191 us vs 110 us), although it is faster in isolation
-  // (profiles/r01_final_bench_n8_cta128.json vs r01_v2_bench_n8.json).  b2d_ctx_set_max_ctas raises it.
+  // 64 CTAs: inside a training step a larger grid waits longer for SMs to drain from the backward kernels than
+  // it gains, although it is faster in isolation.  b2d_ctx_set_max_ctas raises it.
   int max_ctas = 64;
   int tma_ctas = 48;        // CTAs of the TMA-staged kernel (b2d_ctx_set_max_ctas caps it too)
   int tma_ctas_user = 0;
@@ -401,9 +400,9 @@ int pick_algo(b2d_ctx* ctx, size_t n, int wire, int algo) {
   const size_t wire_bytes = n * (wire == B2D_WIRE_BF16 ? 2 : 4);
   const int W = ctx->world;
   const bool nvls = ctx->mc_bound && ctx->nvls_auto && W >= 4;
-  // Small buckets: one kernel, one barrier, every rank reads everything.  Measured cross-over on B200s behind an
-  // NVSwitch (profiles/r02_sweep_{2gpu_v2,4,8}.jsonl): 16 MiB at world 2 (same bytes as any two-shot scheme),
-  // 4 MiB at world 4, 1 MiB at world 8.
+  // Small buckets: one kernel, one barrier, every rank reads everything.  Cross-over: 16 MiB at world 2 (the
+  // same bytes as any two-shot scheme), 4 MiB at world 4, 1 MiB at world 8; b2d_ctx_set_one_shot_max_bytes
+  // overrides it for a given fabric.
   size_t one_shot_max = ctx->one_shot_max_bytes;
   if (!ctx->one_shot_max_user) one_shot_max = W == 2 ? (16u << 20) : (W <= 4 ? (4u << 20) : (1u << 20));
   if (ctx->auto_profile == B2D_PROFILE_LATENCY) {
@@ -415,8 +414,7 @@ int pick_algo(b2d_ctx* ctx, size_t n, int wire, int algo) {
   }
   // B2D_PROFILE_OVERLAP (default; the DDP hook): the exchange shares the GPU with backward kernels.  The staged
   // pipeline's streaming kernels never spin and its exchange kernel holds a few half-SMs only, which is worth more
-  // than the ~10 us it loses in isolation: ResNet-50 on 8 x B200 29.8k img/s against 28.0k with the fused two-shot
-  // (round 1) and 27.3k with NCCL's bf16 hook (profiles/r02_v1_bench_n8*.json).
+  // inside a training step than the few microseconds of extra launches it loses in isolation.
   if (wire_bytes <= (W == 2 ? one_shot_max : (one_shot_max < (1u << 20) ? one_shot_max : (1u << 20)))) return B2D_ALGO_ONE_SHOT;
   // the in-switch reduction pays from 4 ranks up ((1 + 1/W) N w bytes per direction instead of 2 (W-1)/W N w)
   return nvls ? B2D_ALGO_NVLS : B2D_ALGO_STAGED;
@@ -444,15 +442,14 @@ int exch_grid(const b2d_ctx* ctx, size_t chunk_packs, int algo) {
   const size_t per_thread = algo == B2D_ALGO_NVLS ? 8 : (ctx->world <= 8 && kMaxLoadsInFlight / ctx->world > 1 ? kMaxLoadsInFlight / ctx->world : 1);
   size_t grid = (slice + kExThreads * per_thread - 1) / (kExThreads * per_thread);
   if (grid < 1) grid = 1;
-  // multimem keeps the link busy from fewer CTAs (8 x B200, 256 MiB: 790 us with 32 CTAs, 835 with 64)
+  // multimem keeps the link busy from fewer CTAs: NVLS uses half the P2P budget
   const size_t cap = algo == B2D_ALGO_NVLS ? static_cast<size_t>(ctx->exch_ctas > 1 ? ctx->exch_ctas / 2 : 1) : static_cast<size_t>(ctx->exch_ctas);
   if (grid > cap) grid = cap;
   return static_cast<int>(grid);
 }
 
 // S / U: plain streaming kernels.  At most ONE wave (4 CTAs of 256 threads per SM, __launch_bounds__(256, 4)): a grid a
-// few CTAs larger than the machine holds costs a whole second wave — ncu on a 7.5 M-element bucket showed 462 CTAs
-// against 444 slots and 23 us where K0 moves the same bytes in 11 (profiles/r02_ncu_staged_full.md).
+// few CTAs larger than the machine holds costs a whole second wave, which roughly doubles the pass.
 int stream_grid(const b2d_ctx* ctx, size_t packs) {
   size_t grid = (packs + kStThreads * 8 - 1) / (kStThreads * 8);
   if (grid < 1) grid = 1;
@@ -895,8 +892,8 @@ int b2d_ctx_create(int rank, int world, int device, size_t arena_bytes, unsigned
   if (device < 0 || device >= ndev) return fail(nullptr, B2D_ERR_INVALID, "device %d out of range (%d visible)", device, ndev);
   cudaDeviceProp prop;
   B2D_CUDA(nullptr, cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 10)
-    return fail(nullptr, B2D_ERR_UNSUPPORTED, "libb2d is built for sm_100a; device %d is sm_%d%d", device, prop.major, prop.minor);
+  if (prop.major != 9 || prop.minor != 0)
+    return fail(nullptr, B2D_ERR_UNSUPPORTED, "libb2d is built for sm_90a; device %d is sm_%d%d", device, prop.major, prop.minor);
 
   DeviceGuard guard(device);
   if (!guard.ok) return fail(nullptr, B2D_ERR_CUDA, "cudaSetDevice(%d) failed", device);
@@ -1683,8 +1680,7 @@ int b2d_adam_push(b2d_ctx* ctx, float* params, float* exp_avg, float* exp_avg_sq
     B2D_CUDA(ctx, cudaEventRecord(e, static_cast<cudaStream_t>(wait_stream)));
     B2D_CUDA(ctx, cudaStreamWaitEvent(ctx->s_xfer, e, 0));
     // the step is not overlapped with anything and moves 28 B of local HBM traffic per owned element: one full wave
-    // (3 CTAs of 256 threads x 80 registers per SM) instead of the 128 CTAs the first version used (ncu: 12 % of the
-    // warp slots active, 1.3 TB/s; profiles/r02_ncu_owner_full.md)
+    // (3 CTAs of 256 threads x 68 registers per SM on sm_90a); a 128-CTA grid leaves most warp slots idle
     size_t grid = (static_cast<size_t>(P.hi - P.lo) / 4 + kExThreads * 2 - 1) / (kExThreads * 2);
     if (grid < 1) grid = 1;
     const size_t push_cap = static_cast<size_t>(ctx->sm_count) * 3;

@@ -4,8 +4,8 @@
 // no contraction anywhere, so no tensor-core path.  Design rules followed:
 //   * every global access is a 16-byte vector access, warp-contiguous (coalesced);
 //   * loads are issued in explicit batches (up to 16 x 16 B per thread in flight) BEFORE any
-//     of them is consumed: a peer load over NVLink has ~2 us latency, so bandwidth needs
-//     ~1.5 MB in flight per GPU (775 GB/s x 2 us);
+//     of them is consumed: a peer load over NVLink takes microseconds, so bandwidth needs
+//     about a megabyte in flight per GPU (NVLink 4 on H100: 450 GB/s per direction x ~2 us);
 //   * the same (block, thread) touches the same pack in every phase, so one *per-block*
 //     inter-GPU barrier between phases is enough — blocks of one rank never wait for each
 //     other, and a comm kernel can run on a handful of SMs next to the backward pass;
@@ -394,8 +394,8 @@ __global__ void __launch_bounds__(kThreads, 1) k2_two_shot_kernel(const __grid_c
     }
   };
   // phase 2: all-gather + fp32 write-back after ONE barrier.  (An arrival-order variant — gather whichever
-  // peers have finished first, barrier_arrive/poll_arrived in b2d_device.cuh — was measured on 8 GPUs and
-  // lost: every extra round pays a full NVLink round trip; profiles/r01_v4_sweep_8_arrival_order.jsonl.)
+  // peers have finished first, barrier_arrive/poll_arrived in b2d_device.cuh — loses: every extra round pays
+  // a full NVLink round trip.)
   block_barrier(P.peers, P.rank, world, P.timeout_ns, P.diag);
   trace_stamp(P.trace, 4);
   gather(world >= 32 ? 0xffffffffu : ((1u << world) - 1u));

@@ -11,9 +11,8 @@
 //     W  wait_kernel     1 warp  waits until published[r] >= epoch for every r
 //     U  unstage_kernel  local   wire format in the own arena -> fp32 gradients
 //
-// Why this shape (round-1 verdict: the fused K2 ran its phases strictly one after the other — 890 us where the
-// link alone needs 610 us at 256 MiB — and inside a training step its 64 x 512-thread CTAs sat spinning on
-// whole SMs, 330 us per bucket against 107 us isolated):
+// Why this shape (the fused K2 runs its phases strictly one after the other, and inside a training step its
+// 64 x 512-thread CTAs sit spinning on whole SMs while they wait for slower peers):
 //   * the HBM-bound passes (S, U) are plain grid-wide streaming kernels that hold SMs for microseconds and
 //     never spin; only X (a few dozen CTAs) and W (one warp) ever wait for a peer;
 //   * S, X and W+U run on three internal streams, so chunk c+1 is staged and chunk c-1 is written back while
@@ -35,8 +34,8 @@ namespace b2d {
 
 constexpr int kStThreads = 256;   // S / U: plain streaming CTAs
 // X: 256 threads x <= 128 registers = half an SM's register file.  A 512-thread / 128-register CTA needs an EMPTY SM,
-// which never comes up while the stage kernel of the next chunk (or a backward kernel) keeps refilling SMs: measured
-// on 2 x B200 the pipeline then degenerated to stage-all | exchange-all (profiles/r02_tune_2gpu_v1.jsonl).
+// which never comes up while the stage kernel of the next chunk (or a backward kernel) keeps refilling SMs: the
+// pipeline then degenerates to stage-all | exchange-all.
 constexpr int kExThreads = 256;
 
 // spin until *ptr >= target (wrap-safe); trap with diagnostics after timeout_ns
@@ -264,7 +263,7 @@ __global__ void __launch_bounds__(32) wait_published_kernel(const __grid_constan
 }
 
 // ---- link probe: what one GPU can pull from ONE peer with this library's access pattern ------------------
-// (the measured NVLink roofline denominator that bench.py reports next to the nominal 900 GB/s)
+// (the measured NVLink roofline denominator that bench.py reports next to the nominal rate)
 __global__ void __launch_bounds__(kExThreads) peer_read_kernel(const uint4* __restrict__ src, uint4* __restrict__ dst, size_t npacks) {
   constexpr int U = 16;
   const size_t gt = static_cast<size_t>(gridDim.x) * blockDim.x;

@@ -1,10 +1,10 @@
 // b2d_tma.cuh — K2T: the two-shot allreduce with TMA bulk staging through shared memory.
 //
 // Why: the load/store kernels (b2d_kernels.cuh) are capped by what one SM's LSU/L1 can keep in
-// flight (~64 GB/s per SM measured, profiles/r01_v2_trace_sweep_8.jsonl), so they need 64-128 SMs
-// to run the HBM phases at speed.  Here every load is a `cp.async.bulk` (SASS: UBLKCP) issued by one
-// thread into a 3-deep shared-memory ring: up to 192 KiB in flight per SM with no registers and no
-// L1 miss slots, so a few dozen CTAs saturate NVLink (peer loads, ~2.5 us latency) and HBM, and
+// flight, so they need many SMs to run the HBM phases at speed.  Here every load is a
+// `cp.async.bulk` (Hopper TMA, SASS: UBLKCP) issued by one thread into a 3-deep shared-memory ring:
+// 192 KiB in flight per SM (within sm_90's 227 KiB per block) with no registers and no L1 miss
+// slots, so a few dozen CTAs can keep NVLink (peer loads, microseconds of latency) and HBM busy while
 // the rest of the chip keeps running backward kernels.  Results leave with plain 16-byte stores
 // (fire-and-forget, no latency to hide).
 //

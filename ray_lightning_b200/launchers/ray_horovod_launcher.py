@@ -2,7 +2,7 @@
 
 The reference's Horovod launcher (ray_lightning/launchers/ray_horovod_launcher.py:37-277) drives
 ``horovod.ray.RayExecutor`` and calls ``hvd.init()`` in each worker (:192).  Horovod is not
-installable in this image and is OUT OF SCOPE for the B200 data path (SURVEY.md §2.1 row 5b):
+installable in this image and is OUT OF SCOPE for the GPU data path (SURVEY.md §2.1 row 5b):
 its gradient sync is a per-parameter allreduce-average — the same arithmetic contract
 ``RayStrategy``'s libb2d hook implements — so a Horovod user switches to ``RayStrategy``.  The
 class keeps the reference's constructor and ``launch`` signature and fails loudly if used

@@ -5,7 +5,7 @@ attributes, properties and overridden hooks, so ``Trainer(strategy=RayStrategy(.
 same.  What differs is underneath the ``**ddp_kwargs`` pass-through (reference :75,112-116): when
 ``use_gpu`` is set and the caller did not bring a comm hook of their own, the strategy registers
 ``b200_allreduce_hook`` through the SAME seam PL offers for ``ddp_comm_hook`` — so every bucket
-the Reducer finishes goes to one fused sm_100a kernel instead of cast + div + ncclAllReduce +
+the Reducer finishes goes to one fused sm_90a kernel instead of cast + div + ncclAllReduce +
 copy.  New knobs ride in as keyword arguments prefixed ``b200_`` and never reach
 ``DistributedDataParallel``:
 
@@ -213,7 +213,7 @@ class RayStrategy(DDPSpawnStrategy):
         if state is not None and hasattr(state, "total_grad_elems") and state.total_grad_elems is None:
             state.total_grad_elems = sum(p.numel() for p in self.model.parameters() if p.requires_grad)
         if state is not None and hasattr(state, "ensure") and self.root_device.type != "cuda" and self.use_gpu:
-            raise RuntimeError("RayStrategy(use_gpu=True) needs a CUDA device in the worker: the B200 gradient-sync "
+            raise RuntimeError("RayStrategy(use_gpu=True) needs a CUDA device in the worker: the H100 gradient-sync "
                                "path has no CPU fallback")
         super()._register_ddp_hooks()
         # f-3: the per-forward buffer broadcast (BatchNorm statistics ...) goes through the arena too

@@ -3,7 +3,7 @@ optimizer step, parameters pushed back to every rank.
 
 What ``RayShardedStrategy`` (ray_lightning/ray_ddp_sharded.py:12-13) gets from FairScale —
 ``ShardedDataParallel`` reducing every gradient bucket to its owner from the autograd hooks and ``OSS``
-stepping the owned shard and broadcasting it — is laid out here B200-first:
+stepping the owned shard and broadcasting it — is laid out here GPU-first:
 
 * all trainable parameters live in ONE flat fp32 buffer inside the symmetric arena, grouped by owner rank and,
   inside a rank, by optimizer parameter group; gradients accumulate into a second flat buffer (``param.grad``

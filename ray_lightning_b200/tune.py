@@ -1,6 +1,6 @@
 """Ray Tune integration surface (ray_lightning/tune.py:13-241).
 
-OUT OF SCOPE for the B200 data path (HPO control plane; SURVEY.md §2.1 row 9).  ``ray.tune`` is
+OUT OF SCOPE for the GPU data path (HPO control plane; SURVEY.md §2.1 row 9).  ``ray.tune`` is
 not installable here, so — like the reference when Tune is missing (ray_lightning/tune.py:13-27,
 238-241) — the callbacks resolve to ``Unavailable`` and ``is_session_enabled()`` is False.  The
 worker->driver queue they would use (session.py, util.process_results) is implemented and tested.

@@ -1,4 +1,4 @@
-"""Kernel micro-benchmarks (CUDA events, L2-flush between iterations). Not the driver's bench.py.
+"""Kernel micro-benchmarks (CUDA events, L2-flush between iterations); the training benchmark is bench.py.
 
   python tools/microbench.py k0            # world=1 cast/scale kernel, HBM roofline
   python tools/microbench.py loopback      # W ranks on one GPU (protocol overhead only, no NVLink)
@@ -20,7 +20,7 @@ def peaks():
     try:
         return json.load(open(p))
     except Exception:
-        return {"hbm_gbs": 6650.0, "fallback": True}
+        return {"hbm_gbs": 3350.0, "fallback": True}   # H100 SXM data sheet
 
 
 def time_ms(fn, iters, flush=None):
@@ -41,7 +41,7 @@ def time_ms(fn, iters, flush=None):
 def k0():
     hbm = peaks()["hbm_gbs"]
     ctx = _b2d.Context(0, 1, 0, 1 << 20)
-    flush = torch.empty(256 << 20, dtype=torch.float32, device="cuda")  # 1 GiB > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.float32, device="cuda")  # 1 GiB > 50 MB L2
     st = torch.cuda.current_stream()
     for mib in (1, 8, 30, 98, 418, 1354):
         n = mib * (1 << 20) // 4
@@ -176,7 +176,7 @@ def tune():
 
 def ncu_target():
     """A tiny multi-rank workload meant to run with EVERY rank under its own ncu (single-pass metrics, no kernel
-    replay): a few allreduce calls of one size.  See tools/gpu_runs/ncu_multirank.sh."""
+    replay): a few allreduce calls of one size."""
     import torch.distributed as dist
     from ray_lightning_b200.comm import Communicator
     rank, world = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"])
