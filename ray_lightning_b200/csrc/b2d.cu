@@ -21,6 +21,7 @@
 #include "b2d_tma.cuh"
 #include "b2d_staged.cuh"
 #include "b2d_owner.cuh"
+#include "b2d_launch.cuh"
 
 using namespace b2d;
 
@@ -306,56 +307,75 @@ void vmm_unmap(unsigned char* p, size_t bytes) {
   g_drv.MemAddressFree(reinterpret_cast<CUdeviceptr>(p), bytes);
 }
 
-void resolve_timing(b2d_ctx* ctx, bool block) {
+using TimingPair = std::pair<cudaEvent_t, cudaEvent_t>;
+
+// Adds the finished pairs of `pending` to (count, ms) and returns them to the free list; `block` waits for all of them.
+void resolve_pairs(b2d_ctx* ctx, std::vector<TimingPair>& pending, uint64_t& count, double& total_ms, bool block) {
   size_t keep = 0;
-  for (size_t i = 0; i < ctx->ev_pending.size(); ++i) {
-    auto& pr = ctx->ev_pending[i];
+  for (size_t i = 0; i < pending.size(); ++i) {
+    TimingPair& pr = pending[i];
     cudaError_t q = block ? cudaEventSynchronize(pr.second) : cudaEventQuery(pr.second);
     if (q == cudaSuccess) {
       float ms = 0.f;
       if (cudaEventElapsedTime(&ms, pr.first, pr.second) == cudaSuccess) {
-        ctx->timed_ms += ms;
-        ctx->timed_launches += 1;
+        total_ms += ms;
+        count += 1;
       } else {
         cudaGetLastError();
       }
       ctx->ev_free.push_back(pr);
     } else {
-      if (q != cudaErrorNotReady) cudaGetLastError(); else cudaGetLastError();
-      ctx->ev_pending[keep++] = pr;
+      cudaGetLastError();
+      pending[keep++] = pr;
     }
   }
-  ctx->ev_pending.resize(keep);
+  pending.resize(keep);
+}
+
+void resolve_timing(b2d_ctx* ctx, bool block) {
+  resolve_pairs(ctx, ctx->ev_pending, ctx->timed_launches, ctx->timed_ms, block);
+  resolve_pairs(ctx, ctx->exch_pending, ctx->exch_timed, ctx->exch_ms, block);
+}
+
+// A free pair of timing events.  Once 8192 pairs are unresolved, the work goes untimed rather than growing the pool.
+bool take_timing_pair(b2d_ctx* ctx, TimingPair* out) {
+  if (ctx->ev_free.empty() && ctx->ev_pending.size() + ctx->exch_pending.size() >= 8192) resolve_timing(ctx, false);
+  if (ctx->ev_free.empty()) {
+    if (ctx->ev_pending.size() + ctx->exch_pending.size() >= 8192) return false;
+    cudaEvent_t a, b;
+    if (cudaEventCreate(&a) != cudaSuccess) { cudaGetLastError(); return false; }
+    if (cudaEventCreate(&b) != cudaSuccess) { cudaGetLastError(); cudaEventDestroy(a); return false; }
+    ctx->ev_free.emplace_back(a, b);
+  }
+  *out = ctx->ev_free.back();
+  ctx->ev_free.pop_back();
+  return true;
+}
+
+// `waiter` runs what is issued to it next only after everything already issued to `waited`.
+int stream_wait(b2d_ctx* ctx, cudaStream_t waiter, cudaStream_t waited) {
+  cudaEvent_t e = ctx->wait_ev[ctx->wait_ev_idx++ % 8];
+  B2D_CUDA(ctx, cudaEventRecord(e, waited));
+  B2D_CUDA(ctx, cudaStreamWaitEvent(waiter, e, 0));
+  return B2D_OK;
 }
 
 // Everything a launch needs around the kernel itself: stream dependency + optional timing.
 struct LaunchScope {
   b2d_ctx* ctx;
   cudaStream_t comm;
-  std::pair<cudaEvent_t, cudaEvent_t> ev{nullptr, nullptr};
+  TimingPair ev{nullptr, nullptr};
   bool timing = false;
   int begin(void* wait_stream, void* comm_stream) {
     comm = static_cast<cudaStream_t>(comm_stream);
     cudaStream_t ws = static_cast<cudaStream_t>(wait_stream);
     if (ws != comm) {
-      cudaEvent_t e = ctx->wait_ev[ctx->wait_ev_idx++ % 8];
-      B2D_CUDA(ctx, cudaEventRecord(e, ws));
-      B2D_CUDA(ctx, cudaStreamWaitEvent(comm, e, 0));
+      int rc = stream_wait(ctx, comm, ws);
+      if (rc != B2D_OK) return rc;
     }
-    if (ctx->flags & B2D_FLAG_TIMING) {
-      if (ctx->ev_free.empty() && ctx->ev_pending.size() >= 4096) resolve_timing(ctx, false);
-      if (ctx->ev_free.empty() && ctx->ev_pending.size() < 4096) {
-        cudaEvent_t a, b;
-        B2D_CUDA(ctx, cudaEventCreate(&a));
-        B2D_CUDA(ctx, cudaEventCreate(&b));
-        ctx->ev_free.emplace_back(a, b);
-      }
-      if (!ctx->ev_free.empty()) {
-        ev = ctx->ev_free.back();
-        ctx->ev_free.pop_back();
-        timing = true;
-        B2D_CUDA(ctx, cudaEventRecord(ev.first, comm));
-      }
+    if ((ctx->flags & B2D_FLAG_TIMING) && take_timing_pair(ctx, &ev)) {
+      timing = true;
+      B2D_CUDA(ctx, cudaEventRecord(ev.first, comm));
     }
     return B2D_OK;
   }
@@ -371,19 +391,24 @@ struct LaunchScope {
   }
 };
 
-ArParams make_ar_params(b2d_ctx* ctx) {
-  ArParams P{};
-  P.rank = ctx->rank;
-  P.world = ctx->world;
-  P.timeout_ns = static_cast<unsigned long long>(ctx->timeout_ms) * 1000000ull;
-  P.diag = ctx->diag_dev;
-  P.peers = ctx->peers;
-  P.trace = nullptr;
-  return P;
+// The fields of a kernel's parameters that let it wait for peers: who is who, and the watchdog.
+template <typename Params>
+void set_peer_wait(const b2d_ctx* ctx, Params* P) {
+  P->rank = ctx->rank;
+  P->world = ctx->world;
+  P->peers = ctx->peers;
+  P->timeout_ns = static_cast<unsigned long long>(ctx->timeout_ms) * 1000000ull;
+  P->diag = ctx->diag_dev;
+}
+
+// ceil(work / per_cta) CTAs, at least one, at most cap
+int clamp_grid(size_t work, size_t per_cta, size_t cap) {
+  return static_cast<int>(std::min(std::max<size_t>((work + per_cta - 1) / per_cta, 1), cap));
 }
 
 int launch_barrier(b2d_ctx* ctx, cudaStream_t stream) {
-  ArParams P = make_ar_params(ctx);
+  ArParams P{};
+  set_peer_wait(ctx, &P);
   barrier_kernel<<<B2D_MAX_BLOCKS, 32, 0, stream>>>(P);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return fail(ctx, B2D_ERR_CUDA, "barrier launch failed: %s", cudaGetErrorString(e));
@@ -440,22 +465,15 @@ size_t staged_chunk_packs(const b2d_ctx* ctx) {
 int exch_grid(const b2d_ctx* ctx, size_t chunk_packs, int algo) {
   const size_t slice = (chunk_packs + ctx->world - 1) / ctx->world;
   const size_t per_thread = algo == B2D_ALGO_NVLS ? 8 : (ctx->world <= 8 && kMaxLoadsInFlight / ctx->world > 1 ? kMaxLoadsInFlight / ctx->world : 1);
-  size_t grid = (slice + kExThreads * per_thread - 1) / (kExThreads * per_thread);
-  if (grid < 1) grid = 1;
   // multimem keeps the link busy from fewer CTAs: NVLS uses half the P2P budget
   const size_t cap = algo == B2D_ALGO_NVLS ? static_cast<size_t>(ctx->exch_ctas > 1 ? ctx->exch_ctas / 2 : 1) : static_cast<size_t>(ctx->exch_ctas);
-  if (grid > cap) grid = cap;
-  return static_cast<int>(grid);
+  return clamp_grid(slice, kExThreads * per_thread, cap);
 }
 
 // S / U: plain streaming kernels.  At most ONE wave (4 CTAs of 256 threads per SM, __launch_bounds__(256, 4)): a grid a
 // few CTAs larger than the machine holds costs a whole second wave, which roughly doubles the pass.
 int stream_grid(const b2d_ctx* ctx, size_t packs) {
-  size_t grid = (packs + kStThreads * 8 - 1) / (kStThreads * 8);
-  if (grid < 1) grid = 1;
-  const size_t cap = static_cast<size_t>(ctx->sm_count) * 4;
-  if (grid > cap) grid = cap;
-  return static_cast<int>(grid);
+  return clamp_grid(packs, kStThreads * 8, static_cast<size_t>(ctx->sm_count) * 4);
 }
 
 int pick_grid(b2d_ctx* ctx, size_t n, int wire, int algo) {
@@ -467,17 +485,11 @@ int pick_grid(b2d_ctx* ctx, size_t n, int wire, int algo) {
   }
   if (algo == B2D_ALGO_TWO_SHOT_TMA) {
     const size_t slice = (npacks + ctx->world - 1) / ctx->world;
-    size_t grid = (slice + 255) / 256;   // at least 4 KiB of wire per block and slice
-    if (grid < 1) grid = 1;
-    if (grid > static_cast<size_t>(ctx->tma_ctas)) grid = ctx->tma_ctas;
-    return static_cast<int>(grid);
+    return clamp_grid(slice, 256, ctx->tma_ctas);   // at least 4 KiB of wire per block and slice
   }
   size_t work = npacks;
   if (algo != B2D_ALGO_ONE_SHOT) work = (npacks + ctx->world - 1) / ctx->world;
-  size_t grid = (work + kThreads - 1) / kThreads;
-  if (grid < 1) grid = 1;
-  if (grid > static_cast<size_t>(ctx->max_ctas)) grid = ctx->max_ctas;
-  return static_cast<int>(grid);
+  return clamp_grid(work, kThreads, ctx->max_ctas);
 }
 
 // ---- ordering events of the staged exchange ----------------------------------------------------------------
@@ -500,6 +512,17 @@ int ensure_streams(b2d_ctx* ctx) {
   B2D_CUDA(ctx, cudaStreamCreateWithPriority(&ctx->s_stage, cudaStreamNonBlocking, lower));
   B2D_CUDA(ctx, cudaStreamCreateWithPriority(&ctx->s_xfer, cudaStreamNonBlocking, hi));
   B2D_CUDA(ctx, cudaStreamCreateWithPriority(&ctx->s_unstage, cudaStreamNonBlocking, lower));
+  return B2D_OK;
+}
+
+// The final join of the internal streams: `comm` waits for everything issued to s_unstage, and last_unstage_ev marks
+// that point for get_slot's drain.
+int join_unstage(b2d_ctx* ctx, cudaStream_t comm) {
+  cudaEvent_t ed = next_event(ctx);
+  B2D_CUDA(ctx, cudaEventRecord(ed, ctx->s_unstage));
+  B2D_CUDA(ctx, cudaStreamWaitEvent(comm, ed, 0));
+  if (ctx->last_unstage_ev == nullptr) B2D_CUDA(ctx, cudaEventCreateWithFlags(&ctx->last_unstage_ev, cudaEventDisableTiming));
+  B2D_CUDA(ctx, cudaEventRecord(ctx->last_unstage_ev, ctx->s_unstage));
   return B2D_OK;
 }
 
@@ -588,30 +611,15 @@ int get_slot(b2d_ctx* ctx, int key, size_t half_bytes, size_t n, int wire, int a
 
 template <bool BF16, bool NVLS>
 void launch_two_shot(const ArParams& P, int world, int grid, cudaStream_t st) {
-  switch (world) {
-    case 2: k2_two_shot_kernel<2, BF16, NVLS><<<grid, kThreads, 0, st>>>(P); break;
-    case 4: k2_two_shot_kernel<4, BF16, NVLS><<<grid, kThreads, 0, st>>>(P); break;
-    case 8: k2_two_shot_kernel<8, BF16, NVLS><<<grid, kThreads, 0, st>>>(P); break;
-    default: k2_two_shot_kernel<0, BF16, NVLS><<<grid, kThreads, 0, st>>>(P); break;
-  }
+  dispatch_world(world, [&](auto w) { k2_two_shot_kernel<decltype(w)::value, BF16, NVLS><<<grid, kThreads, 0, st>>>(P); });
 }
 template <bool BF16>
 void launch_one_shot(const ArParams& P, int world, int grid, cudaStream_t st) {
-  switch (world) {
-    case 2: k1_one_shot_kernel<2, BF16><<<grid, kThreads, 0, st>>>(P); break;
-    case 4: k1_one_shot_kernel<4, BF16><<<grid, kThreads, 0, st>>>(P); break;
-    case 8: k1_one_shot_kernel<8, BF16><<<grid, kThreads, 0, st>>>(P); break;
-    default: k1_one_shot_kernel<0, BF16><<<grid, kThreads, 0, st>>>(P); break;
-  }
+  dispatch_world(world, [&](auto w) { k1_one_shot_kernel<decltype(w)::value, BF16><<<grid, kThreads, 0, st>>>(P); });
 }
 template <bool BF16>
 void launch_sharded(const ShParams& P, int world, int grid, cudaStream_t st) {
-  switch (world) {
-    case 2: k456_sharded_kernel<2, BF16><<<grid, kThreads, 0, st>>>(P); break;
-    case 4: k456_sharded_kernel<4, BF16><<<grid, kThreads, 0, st>>>(P); break;
-    case 8: k456_sharded_kernel<8, BF16><<<grid, kThreads, 0, st>>>(P); break;
-    default: k456_sharded_kernel<0, BF16><<<grid, kThreads, 0, st>>>(P); break;
-  }
+  dispatch_world(world, [&](auto w) { k456_sharded_kernel<decltype(w)::value, BF16><<<grid, kThreads, 0, st>>>(P); });
 }
 
 // CUDA loads kernels lazily; a load can serialise against running work, and these kernels spin on
@@ -621,8 +629,9 @@ void preload_one(K kernel) {
   cudaFuncAttributes a;
   if (cudaFuncGetAttributes(&a, kernel) != cudaSuccess) cudaGetLastError();
 }
-template <int W>
-void preload_world() {
+// one list per kernel family; `w` is a dispatch_world specialisation
+const auto preload_world = [](auto w) {
+  constexpr int W = decltype(w)::value;
   preload_one(k1_one_shot_kernel<W, true>);
   preload_one(k1_one_shot_kernel<W, false>);
   preload_one(k2_two_shot_kernel<W, true, false>);
@@ -632,53 +641,49 @@ void preload_world() {
   preload_one(k2t_two_shot_tma_kernel<W, true>);
   preload_one(k456_sharded_kernel<W, true>);
   preload_one(k456_sharded_kernel<W, false>);
-}
-template <int W>
-void preload_staged() {
+};
+const auto preload_staged = [](auto w) {
+  constexpr int W = decltype(w)::value;
   preload_one(exch_kernel<W, true, false, false>);
   preload_one(exch_kernel<W, true, true, false>);
   preload_one(exch_kernel<W, false, false, false>);
   preload_one(exch_kernel<W, false, true, false>);
   preload_one(exch_kernel<W, false, false, true>);
   preload_one(exch_kernel<W, false, true, true>);
-}
-template <int W>
-void preload_owner() {
+};
+const auto preload_owner = [](auto w) {
+  constexpr int W = decltype(w)::value;
   preload_one(seg_reduce_kernel<W, true, false>); preload_one(seg_reduce_kernel<W, true, true>);
   preload_one(seg_reduce_kernel<W, false, false>); preload_one(seg_reduce_kernel<W, false, true>);
   preload_one(adam_push_kernel<W, false>); preload_one(adam_push_kernel<W, true>);
-}
-template <int W>
-void tma_attr() {
-  if (cudaFuncSetAttribute(k2t_two_shot_tma_kernel<W, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kTmaSmemBytes) != cudaSuccess)
+};
+const auto tma_attr = [](auto w) {
+  if (cudaFuncSetAttribute(k2t_two_shot_tma_kernel<decltype(w)::value, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kTmaSmemBytes) != cudaSuccess)
     cudaGetLastError();
-}
+};
 void preload_kernels() {
-  tma_attr<0>(); tma_attr<2>(); tma_attr<4>(); tma_attr<8>();
-  preload_staged<0>(); preload_staged<2>(); preload_staged<4>(); preload_staged<8>();
+  const int worlds[] = {0, 2, 4, 8};
+  for (int world : worlds) dispatch_world(world, tma_attr);
+  for (int world : worlds) dispatch_world(world, preload_staged);
   preload_one(stage_kernel<true>); preload_one(stage_kernel<false>);
   preload_one(unstage_kernel<true>); preload_one(unstage_kernel<false>);
   preload_one(arrive_kernel); preload_one(wait_published_kernel); preload_one(peer_read_kernel);
   preload_one(seg_stage_kernel<true>); preload_one(seg_stage_kernel<false>);
-  preload_owner<0>(); preload_owner<2>(); preload_owner<4>(); preload_owner<8>();
+  for (int world : worlds) dispatch_world(world, preload_owner);
   preload_one(bucket_optim_kernel);
   preload_one(k0_cast_scale_kernel<true>);
   preload_one(k0_cast_scale_kernel<false>);
   preload_one(barrier_kernel);
-  preload_world<0>();
-  preload_world<2>();
-  preload_world<4>();
-  preload_world<8>();
+  for (int world : worlds) dispatch_world(world, preload_world);
 }
 
 template <bool BF16, bool NVLS, bool INPLACE>
 void launch_exch_w(const ExParams& P, int world, int grid, cudaStream_t st) {
-  switch (world) {
-    case 2: exch_kernel<2, BF16, NVLS, INPLACE><<<grid, kExThreads, 0, st>>>(P); break;
-    case 4: exch_kernel<4, BF16, NVLS, INPLACE><<<grid, kExThreads, 0, st>>>(P); break;
-    case 8: exch_kernel<8, BF16, NVLS, INPLACE><<<grid, kExThreads, 0, st>>>(P); break;
-    default: exch_kernel<0, BF16, NVLS, INPLACE><<<grid, kExThreads, 0, st>>>(P); break;
-  }
+  dispatch_world(world, [&](auto w) { exch_kernel<decltype(w)::value, BF16, NVLS, INPLACE><<<grid, kExThreads, 0, st>>>(P); });
+}
+template <bool BF16, bool NVLS>
+void launch_seg_reduce(const SegParams& P, int world, int grid, cudaStream_t st) {
+  dispatch_world(world, [&](auto w) { seg_reduce_kernel<decltype(w)::value, BF16, NVLS><<<grid, kExThreads, 0, st>>>(P); });
 }
 void launch_exch(const ExParams& P, int world, int grid, bool bf16, bool nvls, bool inplace, cudaStream_t st) {
   if (inplace) {
@@ -688,38 +693,6 @@ void launch_exch(const ExParams& P, int world, int grid, bool bf16, bool nvls, b
   } else {
     if (nvls) launch_exch_w<false, true, false>(P, world, grid, st); else launch_exch_w<false, false, false>(P, world, grid, st);
   }
-}
-
-void resolve_exch_timing(b2d_ctx* ctx, bool block) {
-  size_t keep = 0;
-  for (size_t i = 0; i < ctx->exch_pending.size(); ++i) {
-    auto& pr = ctx->exch_pending[i];
-    cudaError_t q = block ? cudaEventSynchronize(pr.second) : cudaEventQuery(pr.second);
-    if (q == cudaSuccess) {
-      float ms = 0.f;
-      if (cudaEventElapsedTime(&ms, pr.first, pr.second) == cudaSuccess) { ctx->exch_ms += ms; ctx->exch_timed += 1; }
-      else cudaGetLastError();
-      ctx->ev_free.push_back(pr);
-    } else {
-      cudaGetLastError();
-      ctx->exch_pending[keep++] = pr;
-    }
-  }
-  ctx->exch_pending.resize(keep);
-}
-
-bool take_timing_pair(b2d_ctx* ctx, std::pair<cudaEvent_t, cudaEvent_t>* out) {
-  if (ctx->ev_free.empty() && ctx->ev_pending.size() + ctx->exch_pending.size() >= 8192) { resolve_timing(ctx, false); resolve_exch_timing(ctx, false); }
-  if (ctx->ev_free.empty()) {
-    if (ctx->ev_pending.size() + ctx->exch_pending.size() >= 8192) return false;
-    cudaEvent_t a, b;
-    if (cudaEventCreate(&a) != cudaSuccess) { cudaGetLastError(); return false; }
-    if (cudaEventCreate(&b) != cudaSuccess) { cudaGetLastError(); cudaEventDestroy(a); return false; }
-    ctx->ev_free.emplace_back(a, b);
-  }
-  *out = ctx->ev_free.back();
-  ctx->ev_free.pop_back();
-  return true;
 }
 
 // The staged exchange of one bucket (b2d_staged.cuh): S on s_stage, X on s_xfer, W+U on s_unstage, chunk by
@@ -765,14 +738,13 @@ int launch_staged(b2d_ctx* ctx, int key, float* grad, size_t n, int wire, float 
   StParams SP{};
   SP.scale = scale; SP.rank = ctx->rank; SP.world = ctx->world; SP.peers = ctx->peers;
   ExParams XP{};
-  XP.scale = scale; XP.rank = ctx->rank; XP.world = ctx->world; XP.peers = ctx->peers;
-  XP.timeout_ns = static_cast<unsigned long long>(ctx->timeout_ms) * 1000000ull; XP.diag = ctx->diag_dev;
+  XP.scale = scale;
+  set_peer_wait(ctx, &XP);
 
   std::vector<cudaEvent_t> ev_s(nchunks, nullptr), ev_x(nchunks, nullptr);
   if (phases & 1u) {
-    cudaEvent_t e = ctx->wait_ev[ctx->wait_ev_idx++ % 8];
-    B2D_CUDA(ctx, cudaEventRecord(e, wait_s));
-    B2D_CUDA(ctx, cudaStreamWaitEvent(ctx->s_stage, e, 0));
+    rc = stream_wait(ctx, ctx->s_stage, wait_s);
+    if (rc != B2D_OK) return rc;
     if (!inplace && slot->reuse_ev[half] != nullptr) B2D_CUDA(ctx, cudaStreamWaitEvent(ctx->s_stage, slot->reuse_ev[half], 0));
     if (inplace) {
       SP.epoch = epoch0 + static_cast<uint32_t>(nchunks) - 1u;   // the whole bucket is ready at once
@@ -783,12 +755,12 @@ int launch_staged(b2d_ctx* ctx, int key, float* grad, size_t n, int wire, float 
       for (int c = 0; c < nchunks; ++c) ev_s[c] = es;
     } else {
       for (int c = 0; c < nchunks; ++c) {
-        const size_t p0 = static_cast<size_t>(c) * cp, pc = (npacks - p0 < cp) ? npacks - p0 : cp;
-        SP.grad = grad + p0 * epp;
-        SP.n = (p0 + pc) * epp <= n ? pc * epp : n - p0 * epp;
-        SP.wire = reinterpret_cast<uint4*>(ctx->arena + stage_off) + p0;
+        const ChunkSpan cs = chunk_span(c, npacks, cp, n, epp);
+        SP.grad = grad + cs.p0 * epp;
+        SP.n = cs.n;
+        SP.wire = reinterpret_cast<uint4*>(ctx->arena + stage_off) + cs.p0;
         SP.epoch = epoch0 + static_cast<uint32_t>(c);
-        const int grid = stream_grid(ctx, pc);
+        const int grid = stream_grid(ctx, cs.packs);
         if (bf16) stage_kernel<true><<<grid, kStThreads, 0, ctx->s_stage>>>(SP); else stage_kernel<false><<<grid, kStThreads, 0, ctx->s_stage>>>(SP);
         ctx->launches += 1;
         ev_s[c] = next_event(ctx);
@@ -797,17 +769,17 @@ int launch_staged(b2d_ctx* ctx, int key, float* grad, size_t n, int wire, float 
     }
   }
   if (phases & 2u) {
-    std::pair<cudaEvent_t, cudaEvent_t> tp{nullptr, nullptr};
+    TimingPair tp{nullptr, nullptr};
     const bool timing = (ctx->flags & B2D_FLAG_TIMING) && take_timing_pair(ctx, &tp);
     for (int c = 0; c < nchunks; ++c) {
-      const size_t p0 = static_cast<size_t>(c) * cp, pc = (npacks - p0 < cp) ? npacks - p0 : cp;
+      const ChunkSpan cs = chunk_span(c, npacks, cp, n, epp);
       if (ev_s[c] != nullptr && (c == 0 || ev_s[c] != ev_s[c - 1])) B2D_CUDA(ctx, cudaStreamWaitEvent(ctx->s_xfer, ev_s[c], 0));
       if (timing && c == 0) B2D_CUDA(ctx, cudaEventRecord(tp.first, ctx->s_xfer));
-      XP.wire_off = stage_off + p0 * 16;
-      XP.npacks = pc;
-      XP.n_valid = inplace ? (n - p0 * 4 < pc * 4 ? n - p0 * 4 : pc * 4) : 0;
+      XP.wire_off = stage_off + cs.p0 * 16;
+      XP.npacks = cs.packs;
+      XP.n_valid = inplace ? cs.n_valid : 0;
       XP.epoch = epoch0 + static_cast<uint32_t>(c);
-      const int grid = exch_grid(ctx, pc, algo);
+      const int grid = exch_grid(ctx, cs.packs, algo);
       launch_exch(XP, ctx->world, grid, bf16, nvls, inplace, ctx->s_xfer);
       ctx->launches += 1;
       ctx->exch_launches += 1;
@@ -822,26 +794,23 @@ int launch_staged(b2d_ctx* ctx, int key, float* grad, size_t n, int wire, float 
   }
   if (phases & 4u) {
     for (int c = 0; c < nchunks; ++c) {
-      const size_t p0 = static_cast<size_t>(c) * cp, pc = (npacks - p0 < cp) ? npacks - p0 : cp;
       if (ev_x[c] != nullptr) B2D_CUDA(ctx, cudaStreamWaitEvent(ctx->s_unstage, ev_x[c], 0));
       XP.epoch = epoch0 + static_cast<uint32_t>(c);
       wait_published_kernel<<<1, 32, 0, ctx->s_unstage>>>(XP);
       ctx->launches += 1;
       if (!inplace) {
-        SP.grad = grad + p0 * epp;
-        SP.n = (p0 + pc) * epp <= n ? pc * epp : n - p0 * epp;
-        SP.wire = reinterpret_cast<uint4*>(ctx->arena + stage_off) + p0;
+        const ChunkSpan cs = chunk_span(c, npacks, cp, n, epp);
+        SP.grad = grad + cs.p0 * epp;
+        SP.n = cs.n;
+        SP.wire = reinterpret_cast<uint4*>(ctx->arena + stage_off) + cs.p0;
         SP.epoch = epoch0 + static_cast<uint32_t>(c);
-        const int grid = stream_grid(ctx, pc);
+        const int grid = stream_grid(ctx, cs.packs);
         if (bf16) unstage_kernel<true><<<grid, kStThreads, 0, ctx->s_unstage>>>(SP); else unstage_kernel<false><<<grid, kStThreads, 0, ctx->s_unstage>>>(SP);
         ctx->launches += 1;
       }
     }
-    cudaEvent_t ed = next_event(ctx);
-    B2D_CUDA(ctx, cudaEventRecord(ed, ctx->s_unstage));
-    B2D_CUDA(ctx, cudaStreamWaitEvent(comm, ed, 0));
-    if (ctx->last_unstage_ev == nullptr) B2D_CUDA(ctx, cudaEventCreateWithFlags(&ctx->last_unstage_ev, cudaEventDisableTiming));
-    B2D_CUDA(ctx, cudaEventRecord(ctx->last_unstage_ev, ctx->s_unstage));
+    rc = join_unstage(ctx, comm);
+    if (rc != B2D_OK) return rc;
     if (!inplace) {
       if (slot->reuse_ev[half] == nullptr) B2D_CUDA(ctx, cudaEventCreateWithFlags(&slot->reuse_ev[half], cudaEventDisableTiming));
       B2D_CUDA(ctx, cudaEventRecord(slot->reuse_ev[half], ctx->s_unstage));
@@ -851,6 +820,45 @@ int launch_staged(b2d_ctx* ctx, int key, float* grad, size_t n, int wire, float 
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return fail(ctx, B2D_ERR_CUDA, "kernel launch failed: %s", cudaGetErrorString(e));
   ctx->last_algo = algo; ctx->last_block = kExThreads;
+  return B2D_OK;
+}
+
+void free_tables(b2d_ctx::OwnerBucket& b) { cudaFree(b.d_flat_off); cudaFree(b.d_start); }
+void free_tables(b2d_ctx::OptimBucket& b) { cudaFree(b.d_ptr); cudaFree(b.d_start); }
+
+// Copies a host table to a new device allocation.
+template <typename T>
+int upload_table(b2d_ctx* ctx, const std::vector<T>& v, T** out) {
+  void* p = nullptr;
+  B2D_CUDA(ctx, cudaMalloc(&p, v.size() * sizeof(T)));
+  *out = static_cast<T*>(p);
+  B2D_CUDA(ctx, cudaMemcpy(p, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice));
+  return B2D_OK;
+}
+
+// Forgets bucket `id` of `buckets` before it is registered again.  Its device tables are freed once the device is idle:
+// kernels still in flight may read them.
+template <typename Bucket>
+int drop_bucket(b2d_ctx* ctx, std::map<int, Bucket>& buckets, int id) {
+  auto it = buckets.find(id);
+  if (it == buckets.end()) return B2D_OK;
+  B2D_CUDA(ctx, cudaDeviceSynchronize());
+  free_tables(it->second);
+  buckets.erase(it);
+  return B2D_OK;
+}
+
+// shard_off[0 .. world]: the owner shards of [0, n), non-decreasing multiples of 8.  *max_len: the longest shard.
+int check_shard_off(b2d_ctx* ctx, const int64_t* shard_off, size_t n, size_t* max_len) {
+  if (shard_off[0] != 0 || static_cast<size_t>(shard_off[ctx->world]) != n)
+    return fail(ctx, B2D_ERR_INVALID, "shard_off must start at 0 and end at n");
+  *max_len = 0;
+  for (int r = 0; r < ctx->world; ++r) {
+    if (shard_off[r + 1] < shard_off[r] || shard_off[r] % 8 != 0 || shard_off[r + 1] % 8 != 0)
+      return fail(ctx, B2D_ERR_INVALID, "shard offsets must be non-decreasing multiples of 8 (got %lld..%lld for rank %d)",
+                  (long long)shard_off[r], (long long)shard_off[r + 1], r);
+    *max_len = std::max(*max_len, static_cast<size_t>(shard_off[r + 1] - shard_off[r]));
+  }
   return B2D_OK;
 }
 
@@ -1152,8 +1160,8 @@ int b2d_ctx_destroy(b2d_ctx* ctx) {
     for (auto& pr : ctx->ev_free) { cudaEventDestroy(pr.first); cudaEventDestroy(pr.second); }
     for (auto& e : ctx->wait_ev) if (e != nullptr) cudaEventDestroy(e);
     for (auto& pr : ctx->exch_pending) { cudaEventDestroy(pr.first); cudaEventDestroy(pr.second); }
-    for (auto& kv : ctx->owner_buckets) { cudaFree(kv.second.d_flat_off); cudaFree(kv.second.d_start); }
-    for (auto& kv : ctx->optim_buckets) { cudaFree(kv.second.d_ptr); cudaFree(kv.second.d_start); }
+    for (auto& kv : ctx->owner_buckets) free_tables(kv.second);
+    for (auto& kv : ctx->optim_buckets) free_tables(kv.second);
     for (auto& e : ctx->ev_ring) if (e != nullptr) cudaEventDestroy(e);
     if (ctx->last_unstage_ev != nullptr) cudaEventDestroy(ctx->last_unstage_ev);
     for (auto& kv : ctx->slots) for (cudaEvent_t e : kv.second.reuse_ev) if (e != nullptr) cudaEventDestroy(e);
@@ -1283,9 +1291,7 @@ int b2d_plan(b2d_ctx* ctx, size_t n, int wire, int algo, int* algo_out, int* gri
   const int a = pick_algo(ctx, n, wire, algo);
   int grid;
   if (ctx->world == 1) {
-    size_t g = (n / 4 + static_cast<size_t>(kThreads) * 4 - 1) / (static_cast<size_t>(kThreads) * 4);
-    const size_t cap = static_cast<size_t>(ctx->sm_count) * 4;
-    grid = static_cast<int>(g < 1 ? 1 : (g > cap ? cap : g));
+    grid = clamp_grid(n / 4, static_cast<size_t>(kThreads) * 4, static_cast<size_t>(ctx->sm_count) * 4);
   } else {
     grid = pick_grid(ctx, n, wire, a);
   }
@@ -1338,7 +1344,8 @@ int b2d_allreduce_bucket_phased(b2d_ctx* ctx, int bucket_idx, float* grad, size_
   rc = get_slot(ctx, bucket_idx, half, n, wire, a, grid, comm, &stage_off);
   if (rc != B2D_OK) return rc;
 
-  ArParams P = make_ar_params(ctx);
+  ArParams P{};
+  set_peer_wait(ctx, &P);
   P.grad = grad; P.n = n; P.stage_off = stage_off; P.scale = scale;
   P.trace = ctx->trace_dev;
   ctx->trace_grid = grid;
@@ -1358,12 +1365,7 @@ int b2d_allreduce_bucket_phased(b2d_ctx* ctx, int bucket_idx, float* grad, size_
       break;
     case B2D_ALGO_TWO_SHOT_TMA: {
       const int mt = tma_mt(slice, grid);
-      switch (ctx->world) {
-        case 2: k2t_two_shot_tma_kernel<2, true><<<grid, kTmaThreads, kTmaSmemBytes, comm>>>(P, mt); break;
-        case 4: k2t_two_shot_tma_kernel<4, true><<<grid, kTmaThreads, kTmaSmemBytes, comm>>>(P, mt); break;
-        case 8: k2t_two_shot_tma_kernel<8, true><<<grid, kTmaThreads, kTmaSmemBytes, comm>>>(P, mt); break;
-        default: k2t_two_shot_tma_kernel<0, true><<<grid, kTmaThreads, kTmaSmemBytes, comm>>>(P, mt); break;
-      }
+      dispatch_world(ctx->world, [&](auto w) { k2t_two_shot_tma_kernel<decltype(w)::value, true><<<grid, kTmaThreads, kTmaSmemBytes, comm>>>(P, mt); });
       break;
     }
     default:
@@ -1387,16 +1389,9 @@ static int sharded_common(b2d_ctx* ctx, int slot, const float* grads, float* par
   std::lock_guard<std::mutex> lk(ctx->mu);
   if (shard_off == nullptr) return fail(ctx, B2D_ERR_INVALID, "shard_off is NULL");
   if (wire != B2D_WIRE_FP32 && wire != B2D_WIRE_BF16) return fail(ctx, B2D_ERR_INVALID, "bad wire %d", wire);
-  if (shard_off[0] != 0 || static_cast<size_t>(shard_off[ctx->world]) != n)
-    return fail(ctx, B2D_ERR_INVALID, "shard_off must start at 0 and end at n");
   size_t max_len = 0;
-  for (int r = 0; r < ctx->world; ++r) {
-    if (shard_off[r + 1] < shard_off[r] || shard_off[r] % 8 != 0 || shard_off[r + 1] % 8 != 0)
-      return fail(ctx, B2D_ERR_INVALID, "shard offsets must be non-decreasing multiples of 8 (got %lld..%lld for rank %d)",
-                  (long long)shard_off[r], (long long)shard_off[r + 1], r);
-    const size_t l = static_cast<size_t>(shard_off[r + 1] - shard_off[r]);
-    max_len = l > max_len ? l : max_len;
-  }
+  rc = check_shard_off(ctx, shard_off, n, &max_len);
+  if (rc != B2D_OK) return rc;
   if (n == 0) return B2D_OK;
   DeviceGuard guard(ctx->device);
   if (!guard.ok) return fail(ctx, B2D_ERR_CUDA, "cudaSetDevice(%d) failed", ctx->device);
@@ -1404,12 +1399,11 @@ static int sharded_common(b2d_ctx* ctx, int slot, const float* grads, float* par
 
   ShParams P{};
   P.grads = grads; P.params = params; P.exp_avg = exp_avg; P.exp_avg_sq = exp_avg_sq; P.rs_out = rs_out;
-  P.n = n; P.scale = scale; P.rank = ctx->rank; P.world = ctx->world;
+  P.n = n; P.scale = scale;
   P.do_stage_reduce = do_sr; P.do_adam = adam != nullptr; P.do_gather = do_gather; P.end_barrier = end_barrier;
   for (int r = 0; r <= ctx->world; ++r) P.off[r] = shard_off[r];
   for (int r = ctx->world + 1; r <= B2D_MAX_WORLD; ++r) P.off[r] = shard_off[ctx->world];
-  P.timeout_ns = static_cast<unsigned long long>(ctx->timeout_ms) * 1000000ull;
-  P.diag = ctx->diag_dev; P.peers = ctx->peers;
+  set_peer_wait(ctx, &P);
 
   if (do_gather) {
     const unsigned char* p8 = reinterpret_cast<const unsigned char*>(params);
@@ -1422,48 +1416,32 @@ static int sharded_common(b2d_ctx* ctx, int slot, const float* grads, float* par
     if (adam != nullptr) {
       if (params == nullptr || exp_avg == nullptr || exp_avg_sq == nullptr) return fail(ctx, B2D_ERR_INVALID, "params/exp_avg/exp_avg_sq are NULL");
       if (adam->step < 1) return fail(ctx, B2D_ERR_INVALID, "adam.step must be >= 1");
-      AdamConsts& a = P.adam;
-      a.lr = adam->lr; a.beta1 = adam->beta1; a.beta2 = adam->beta2; a.eps = adam->eps; a.weight_decay = adam->weight_decay;
-      a.one_minus_beta1 = static_cast<float>(1.0 - static_cast<double>(adam->beta1));
-      a.one_minus_beta2 = static_cast<float>(1.0 - static_cast<double>(adam->beta2));
-      // python-float (double) arithmetic of torch/optim/adam.py:503-541, cast once
-      double bc1 = 1.0, bc2 = 1.0, b1p = 1.0, b2p = 1.0;
-      for (int i = 0; i < adam->step; ++i) { b1p *= static_cast<double>(adam->beta1); b2p *= static_cast<double>(adam->beta2); }
-      bc1 = 1.0 - b1p; bc2 = 1.0 - b2p;
-      a.step_size = static_cast<float>(static_cast<double>(adam->lr) / bc1);
-      a.inv_bc2_sqrt = 1.0f / static_cast<float>(sqrt(bc2));
-      a.decay_mul = static_cast<float>(1.0 - static_cast<double>(adam->lr) * static_cast<double>(adam->weight_decay));
-      a.adamw = adam->adamw;
+      P.adam = adam_consts(*adam);
       if (adam->zero_grads) P.grads_rw = const_cast<float*>(grads);
     } else if (rs_out == nullptr) {
       return fail(ctx, B2D_ERR_INVALID, "reduce-scatter output is NULL");
     }
     const size_t half = n * (wire == B2D_WIRE_BF16 ? 2 : 4);
-    size_t work = max_len / (wire == B2D_WIRE_BF16 ? 8 : 4);
-    size_t grid = (work + kThreads - 1) / kThreads;
-    if (grid < 1) grid = 1;
-    if (grid > static_cast<size_t>(ctx->max_ctas)) grid = ctx->max_ctas;
+    const int grid = clamp_grid(max_len / (wire == B2D_WIRE_BF16 ? 8 : 4), kThreads, ctx->max_ctas);
     size_t stage_off = 0;
-    rc = get_slot(ctx, 0x40000000 + slot, half, n, wire, 100 + do_gather, static_cast<int>(grid), comm, &stage_off);
+    rc = get_slot(ctx, 0x40000000 + slot, half, n, wire, 100 + do_gather, grid, comm, &stage_off);
     if (rc != B2D_OK) return rc;
     P.stage_off = stage_off;
     LaunchScope ls{ctx};
     rc = ls.begin(wait_stream, comm_stream);
     if (rc != B2D_OK) return rc;
-    if (wire == B2D_WIRE_BF16) launch_sharded<true>(P, ctx->world, static_cast<int>(grid), comm);
-    else launch_sharded<false>(P, ctx->world, static_cast<int>(grid), comm);
-    ctx->last_algo = 10; ctx->last_grid = static_cast<int>(grid); ctx->last_block = kThreads;
+    if (wire == B2D_WIRE_BF16) launch_sharded<true>(P, ctx->world, grid, comm);
+    else launch_sharded<false>(P, ctx->world, grid, comm);
+    ctx->last_algo = 10; ctx->last_grid = grid; ctx->last_block = kThreads;
     return ls.end();
   }
   // all-gather only
-  size_t grid = (max_len / 4 + kThreads - 1) / kThreads;
-  if (grid < 1) grid = 1;
-  if (grid > static_cast<size_t>(ctx->max_ctas)) grid = ctx->max_ctas;
+  const int grid = clamp_grid(max_len / 4, kThreads, ctx->max_ctas);
   LaunchScope ls{ctx};
   rc = ls.begin(wait_stream, comm_stream);
   if (rc != B2D_OK) return rc;
-  launch_sharded<false>(P, ctx->world, static_cast<int>(grid), comm);
-  ctx->last_algo = 11; ctx->last_grid = static_cast<int>(grid); ctx->last_block = kThreads;
+  launch_sharded<false>(P, ctx->world, grid, comm);
+  ctx->last_algo = 11; ctx->last_grid = grid; ctx->last_block = kThreads;
   return ls.end();
 }
 
@@ -1487,82 +1465,27 @@ int b2d_allgather(b2d_ctx* ctx, float* buf, size_t n, const int64_t* shard_off, 
 }
 
 // ---- sharded path on the staged machinery (b2d_owner.cuh) ----------------------------------------------------
-static void fill_adam_consts(const b2d_adam* adam, AdamConsts* a) {
-  a->lr = adam->lr; a->beta1 = adam->beta1; a->beta2 = adam->beta2; a->eps = adam->eps; a->weight_decay = adam->weight_decay;
-  a->one_minus_beta1 = static_cast<float>(1.0 - static_cast<double>(adam->beta1));
-  a->one_minus_beta2 = static_cast<float>(1.0 - static_cast<double>(adam->beta2));
-  // python-float (double) arithmetic of torch/optim/adam.py:503-541, cast once
-  double b1p = 1.0, b2p = 1.0;
-  for (int i = 0; i < adam->step; ++i) { b1p *= static_cast<double>(adam->beta1); b2p *= static_cast<double>(adam->beta2); }
-  a->step_size = static_cast<float>(static_cast<double>(adam->lr) / (1.0 - b1p));
-  a->inv_bc2_sqrt = 1.0f / static_cast<float>(sqrt(1.0 - b2p));
-  a->decay_mul = static_cast<float>(1.0 - static_cast<double>(adam->lr) * static_cast<double>(adam->weight_decay));
-  a->adamw = adam->adamw;
-}
-
 int b2d_bucket_register(b2d_ctx* ctx, int bucket_id, const b2d_seg* segs, int nseg, int wire) {
   int rc = check_ready(ctx);
   if (rc != B2D_OK) return rc;
   std::lock_guard<std::mutex> lk(ctx->mu);
   if (segs == nullptr || nseg < 1) return fail(ctx, B2D_ERR_INVALID, "a reduce bucket needs at least one segment");
   if (wire != B2D_WIRE_FP32 && wire != B2D_WIRE_BF16) return fail(ctx, B2D_ERR_INVALID, "bad wire %d", wire);
-  const long long epp = wire == B2D_WIRE_BF16 ? 8 : 4;
-  std::vector<b2d_seg> v(segs, segs + nseg);
-  for (const b2d_seg& sgm : v) {
-    if (sgm.owner < 0 || sgm.owner >= ctx->world) return fail(ctx, B2D_ERR_INVALID, "segment owner %d out of range", sgm.owner);
-    if (sgm.flat_off < 0 || sgm.len <= 0 || sgm.flat_off % 8 != 0 || sgm.len % 8 != 0)
-      return fail(ctx, B2D_ERR_INVALID, "segments must be non-empty, 8-element aligned runs (got %lld + %lld)", (long long)sgm.flat_off, (long long)sgm.len);
-  }
-  std::stable_sort(v.begin(), v.end(), [](const b2d_seg& a, const b2d_seg& b) { return a.owner != b.owner ? a.owner < b.owner : a.flat_off < b.flat_off; });
-  std::vector<b2d_seg> m;   // merge runs that touch
-  for (const b2d_seg& sgm : v) {
-    if (!m.empty() && m.back().owner == sgm.owner && m.back().flat_off + m.back().len == sgm.flat_off) m.back().len += sgm.len;
-    else m.push_back(sgm);
-  }
-  std::vector<long long> flat(m.size());
-  std::vector<unsigned> start(m.size() + 1, 0);
-  b2d_ctx::OwnerBucket nb;
-  nb.nseg = static_cast<int>(m.size()); nb.wire = wire;
-  unsigned long long cum = 0;
-  int next_owner = 0;
-  for (size_t i = 0; i < m.size(); ++i) {
-    while (next_owner <= m[i].owner) nb.owner_pack[next_owner++] = static_cast<unsigned>(cum);
-    flat[i] = m[i].flat_off;
-    start[i] = static_cast<unsigned>(cum);
-    cum += static_cast<unsigned long long>(m[i].len / epp);
-    if (cum > 0xffffffffull) return fail(ctx, B2D_ERR_INVALID, "reduce bucket too large");
-  }
-  start[m.size()] = static_cast<unsigned>(cum);
-  while (next_owner <= ctx->world) nb.owner_pack[next_owner++] = static_cast<unsigned>(cum);
-  for (int r = ctx->world + 1; r <= B2D_MAX_WORLD; ++r) nb.owner_pack[r] = static_cast<unsigned>(cum);
+  OwnerTable t;
+  const std::string bad = build_owner_table(segs, nseg, ctx->world, wire, &t);
+  if (!bad.empty()) return fail(ctx, B2D_ERR_INVALID, "%s", bad.c_str());
   DeviceGuard guard(ctx->device);
-  auto it = ctx->owner_buckets.find(bucket_id);
-  if (it != ctx->owner_buckets.end()) {
-    B2D_CUDA(ctx, cudaDeviceSynchronize());
-    cudaFree(it->second.d_flat_off); cudaFree(it->second.d_start);
-    ctx->owner_buckets.erase(it);
-  }
-  void *a = nullptr, *b = nullptr;
-  B2D_CUDA(ctx, cudaMalloc(&a, flat.size() * sizeof(long long)));
-  B2D_CUDA(ctx, cudaMalloc(&b, start.size() * sizeof(unsigned)));
-  B2D_CUDA(ctx, cudaMemcpy(a, flat.data(), flat.size() * sizeof(long long), cudaMemcpyHostToDevice));
-  B2D_CUDA(ctx, cudaMemcpy(b, start.data(), start.size() * sizeof(unsigned), cudaMemcpyHostToDevice));
-  nb.d_flat_off = static_cast<long long*>(a); nb.d_start = static_cast<unsigned*>(b);
+  rc = drop_bucket(ctx, ctx->owner_buckets, bucket_id);
+  if (rc != B2D_OK) return rc;
+  b2d_ctx::OwnerBucket nb;
+  nb.nseg = static_cast<int>(t.flat_off.size()); nb.wire = wire;
+  std::copy(t.owner_pack, t.owner_pack + B2D_MAX_WORLD + 1, nb.owner_pack);
+  rc = upload_table(ctx, t.flat_off, &nb.d_flat_off);
+  if (rc == B2D_OK) rc = upload_table(ctx, t.start, &nb.d_start);
+  if (rc != B2D_OK) return rc;
   ctx->owner_buckets[bucket_id] = nb;
   return B2D_OK;
 }
-
-}  // extern "C"
-template <bool BF16, bool NVLS>
-static void launch_seg_reduce(const SegParams& P, int world, int grid, cudaStream_t st) {
-  switch (world) {
-    case 2: seg_reduce_kernel<2, BF16, NVLS><<<grid, kExThreads, 0, st>>>(P); break;
-    case 4: seg_reduce_kernel<4, BF16, NVLS><<<grid, kExThreads, 0, st>>>(P); break;
-    case 8: seg_reduce_kernel<8, BF16, NVLS><<<grid, kExThreads, 0, st>>>(P); break;
-    default: seg_reduce_kernel<0, BF16, NVLS><<<grid, kExThreads, 0, st>>>(P); break;
-  }
-}
-extern "C" {
 
 int b2d_reduce_to_owner(b2d_ctx* ctx, int bucket_id, float* grads, float* reduced, const int64_t* shard_off, float scale,
                         unsigned flags, unsigned phases, void* wait_stream, void* comm_stream) {
@@ -1595,13 +1518,12 @@ int b2d_reduce_to_owner(b2d_ctx* ctx, int bucket_id, float* grads, float* reduce
   for (int r = 0; r <= B2D_MAX_WORLD; ++r) P.owner_pack[r] = ob.owner_pack[r];
   P.grads = grads; P.reduced = reduced; P.shard_lo = shard_off[ctx->rank]; P.wire_off = stage_off; P.scale = scale;
   P.zero_grads = (flags & B2D_RTO_ZERO_GRADS) ? 1 : 0; P.accumulate = (flags & B2D_RTO_ACCUMULATE) ? 1 : 0;
-  P.rank = ctx->rank; P.world = ctx->world; P.epoch = ob.op_epoch;
-  P.timeout_ns = static_cast<unsigned long long>(ctx->timeout_ms) * 1000000ull; P.diag = ctx->diag_dev; P.peers = ctx->peers;
+  P.epoch = ob.op_epoch;
+  set_peer_wait(ctx, &P);
   cudaEvent_t es = nullptr;
   if (phases & 1u) {
-    cudaEvent_t e = ctx->wait_ev[ctx->wait_ev_idx++ % 8];
-    B2D_CUDA(ctx, cudaEventRecord(e, static_cast<cudaStream_t>(wait_stream)));
-    B2D_CUDA(ctx, cudaStreamWaitEvent(ctx->s_stage, e, 0));
+    rc = stream_wait(ctx, ctx->s_stage, static_cast<cudaStream_t>(wait_stream));
+    if (rc != B2D_OK) return rc;
     const int grid = stream_grid(ctx, total);
     if (bf16) seg_stage_kernel<true><<<grid, kStThreads, 0, ctx->s_stage>>>(P); else seg_stage_kernel<false><<<grid, kStThreads, 0, ctx->s_stage>>>(P);
     ctx->launches += 1;
@@ -1612,20 +1534,18 @@ int b2d_reduce_to_owner(b2d_ctx* ctx, int bucket_id, float* grads, float* reduce
     if (es != nullptr) B2D_CUDA(ctx, cudaStreamWaitEvent(ctx->s_xfer, es, 0));
     const size_t mine = ob.owner_pack[ctx->rank + 1] - ob.owner_pack[ctx->rank];
     const size_t per_thread = nvls ? 8 : (kMaxLoadsInFlight / ctx->world > 1 ? kMaxLoadsInFlight / ctx->world : 1);
-    size_t grid = (mine + kExThreads * per_thread - 1) / (kExThreads * per_thread);
-    if (grid < 1) grid = 1;
-    if (grid > static_cast<size_t>(ctx->exch_ctas)) grid = ctx->exch_ctas;
-    std::pair<cudaEvent_t, cudaEvent_t> tp{nullptr, nullptr};
+    const int grid = clamp_grid(mine, kExThreads * per_thread, ctx->exch_ctas);
+    TimingPair tp{nullptr, nullptr};
     const bool timing = (ctx->flags & B2D_FLAG_TIMING) && take_timing_pair(ctx, &tp);
     if (timing) B2D_CUDA(ctx, cudaEventRecord(tp.first, ctx->s_xfer));
-    if (bf16) { if (nvls) launch_seg_reduce<true, true>(P, ctx->world, static_cast<int>(grid), ctx->s_xfer); else launch_seg_reduce<true, false>(P, ctx->world, static_cast<int>(grid), ctx->s_xfer); }
-    else      { if (nvls) launch_seg_reduce<false, true>(P, ctx->world, static_cast<int>(grid), ctx->s_xfer); else launch_seg_reduce<false, false>(P, ctx->world, static_cast<int>(grid), ctx->s_xfer); }
+    if (bf16) { if (nvls) launch_seg_reduce<true, true>(P, ctx->world, grid, ctx->s_xfer); else launch_seg_reduce<true, false>(P, ctx->world, grid, ctx->s_xfer); }
+    else      { if (nvls) launch_seg_reduce<false, true>(P, ctx->world, grid, ctx->s_xfer); else launch_seg_reduce<false, false>(P, ctx->world, grid, ctx->s_xfer); }
     ctx->launches += 1; ctx->exch_launches += 1;
     if (timing) { B2D_CUDA(ctx, cudaEventRecord(tp.second, ctx->s_xfer)); ctx->exch_pending.push_back(tp); }
     cudaEvent_t ex = next_event(ctx);
     B2D_CUDA(ctx, cudaEventRecord(ex, ctx->s_xfer));
     B2D_CUDA(ctx, cudaStreamWaitEvent(comm, ex, 0));
-    ctx->last_grid = static_cast<int>(grid);
+    ctx->last_grid = grid;
     ob.op_epoch = 0;
   }
   cudaError_t e = cudaGetLastError();
@@ -1645,10 +1565,9 @@ int b2d_adam_push(b2d_ctx* ctx, float* params, float* exp_avg, float* exp_avg_sq
   if (ngroups > 0 && (groups == nullptr || exp_avg == nullptr || exp_avg_sq == nullptr || reduced == nullptr))
     return fail(ctx, B2D_ERR_INVALID, "groups / exp_avg / exp_avg_sq / reduced are NULL");
   if ((phases & 6u) == 0 || (phases & ~6u) != 0) return fail(ctx, B2D_ERR_INVALID, "bad phase mask %u (bit 1 step + push, bit 2 wait)", phases);
-  if (shard_off[0] != 0 || static_cast<size_t>(shard_off[ctx->world]) != n) return fail(ctx, B2D_ERR_INVALID, "shard_off must start at 0 and end at n");
-  for (int r = 0; r < ctx->world; ++r)
-    if (shard_off[r + 1] < shard_off[r] || shard_off[r] % 8 != 0 || shard_off[r + 1] % 8 != 0)
-      return fail(ctx, B2D_ERR_INVALID, "shard offsets must be non-decreasing multiples of 8");
+  size_t max_len = 0;
+  rc = check_shard_off(ctx, shard_off, n, &max_len);
+  if (rc != B2D_OK) return rc;
   const bool nvls = (flags & B2D_RTO_NVLS) != 0;
   if (nvls && !ctx->mc_bound) return fail(ctx, B2D_ERR_UNSUPPORTED, "NVLS requested but no multicast object is bound");
   const unsigned char* p8 = reinterpret_cast<const unsigned char*>(params);
@@ -1673,47 +1592,36 @@ int b2d_adam_push(b2d_ctx* ctx, float* params, float* exp_avg, float* exp_avg_sq
         return fail(ctx, B2D_ERR_INVALID, "parameter group %d covers [%lld, %lld) of a shard of %lld elements", k, (long long)groups[k].lo, (long long)groups[k].hi, (long long)(P.hi - P.lo));
       if (groups[k].adam.step < 1) return fail(ctx, B2D_ERR_INVALID, "adam.step must be >= 1");
       P.group_lo[k] = groups[k].lo; P.group_hi[k] = groups[k].hi;
-      fill_adam_consts(&groups[k].adam, &P.group[k]);
+      P.group[k] = adam_consts(groups[k].adam);
     }
     P.rank = ctx->rank; P.world = ctx->world; P.epoch = ctx->push_epoch; P.peers = ctx->peers;
-    cudaEvent_t e = ctx->wait_ev[ctx->wait_ev_idx++ % 8];
-    B2D_CUDA(ctx, cudaEventRecord(e, static_cast<cudaStream_t>(wait_stream)));
-    B2D_CUDA(ctx, cudaStreamWaitEvent(ctx->s_xfer, e, 0));
+    rc = stream_wait(ctx, ctx->s_xfer, static_cast<cudaStream_t>(wait_stream));
+    if (rc != B2D_OK) return rc;
     // the step is not overlapped with anything and moves 28 B of local HBM traffic per owned element: one full wave
     // (3 CTAs of 256 threads x 68 registers per SM on sm_90a); a 128-CTA grid leaves most warp slots idle
-    size_t grid = (static_cast<size_t>(P.hi - P.lo) / 4 + kExThreads * 2 - 1) / (kExThreads * 2);
-    if (grid < 1) grid = 1;
-    const size_t push_cap = static_cast<size_t>(ctx->sm_count) * 3;
-    if (grid > push_cap) grid = push_cap;
-    std::pair<cudaEvent_t, cudaEvent_t> tp{nullptr, nullptr};
+    const int grid = clamp_grid(static_cast<size_t>(P.hi - P.lo) / 4, kExThreads * 2, static_cast<size_t>(ctx->sm_count) * 3);
+    TimingPair tp{nullptr, nullptr};
     const bool timing = (ctx->flags & B2D_FLAG_TIMING) && take_timing_pair(ctx, &tp);
     if (timing) B2D_CUDA(ctx, cudaEventRecord(tp.first, ctx->s_xfer));
-#define B2D_PUSH(WW) { if (nvls) adam_push_kernel<WW, true><<<grid, kExThreads, 0, ctx->s_xfer>>>(P); else adam_push_kernel<WW, false><<<grid, kExThreads, 0, ctx->s_xfer>>>(P); }
-    switch (ctx->world) {
-      case 2: B2D_PUSH(2) break;
-      case 4: B2D_PUSH(4) break;
-      case 8: B2D_PUSH(8) break;
-      default: B2D_PUSH(0) break;
-    }
-#undef B2D_PUSH
+    dispatch_world(ctx->world, [&](auto w) {
+      constexpr int W = decltype(w)::value;
+      if (nvls) adam_push_kernel<W, true><<<grid, kExThreads, 0, ctx->s_xfer>>>(P); else adam_push_kernel<W, false><<<grid, kExThreads, 0, ctx->s_xfer>>>(P);
+    });
     ctx->launches += 1;
     if (timing) { B2D_CUDA(ctx, cudaEventRecord(tp.second, ctx->s_xfer)); ctx->ev_pending.push_back(tp); }
-    ctx->last_grid = static_cast<int>(grid);
+    ctx->last_grid = grid;
   }
   if (phases & 4u) {
     ExParams XP{};
-    XP.rank = ctx->rank; XP.world = ctx->world; XP.peers = ctx->peers; XP.epoch = ctx->push_epoch;
-    XP.timeout_ns = static_cast<unsigned long long>(ctx->timeout_ms) * 1000000ull; XP.diag = ctx->diag_dev;
+    XP.epoch = ctx->push_epoch;
+    set_peer_wait(ctx, &XP);
     cudaEvent_t ex = next_event(ctx);
     B2D_CUDA(ctx, cudaEventRecord(ex, ctx->s_xfer));
     B2D_CUDA(ctx, cudaStreamWaitEvent(ctx->s_unstage, ex, 0));
     wait_published_kernel<<<1, 32, 0, ctx->s_unstage>>>(XP);
     ctx->launches += 1;
-    cudaEvent_t ed = next_event(ctx);
-    B2D_CUDA(ctx, cudaEventRecord(ed, ctx->s_unstage));
-    B2D_CUDA(ctx, cudaStreamWaitEvent(comm, ed, 0));
-    if (ctx->last_unstage_ev == nullptr) B2D_CUDA(ctx, cudaEventCreateWithFlags(&ctx->last_unstage_ev, cudaEventDisableTiming));
-    B2D_CUDA(ctx, cudaEventRecord(ctx->last_unstage_ev, ctx->s_unstage));
+    rc = join_unstage(ctx, comm);
+    if (rc != B2D_OK) return rc;
     ctx->push_epoch = 0;
   }
   cudaError_t e = cudaGetLastError();
@@ -1742,20 +1650,13 @@ int b2d_optim_register(b2d_ctx* ctx, int bucket_id, float* const* params, float*
   }
   start[nparam] = static_cast<unsigned>(cur);
   DeviceGuard guard(ctx->device);
-  auto it = ctx->optim_buckets.find(bucket_id);
-  if (it != ctx->optim_buckets.end()) {
-    B2D_CUDA(ctx, cudaDeviceSynchronize());
-    cudaFree(it->second.d_ptr); cudaFree(it->second.d_start);
-    ctx->optim_buckets.erase(it);
-  }
+  int rc = drop_bucket(ctx, ctx->optim_buckets, bucket_id);
+  if (rc != B2D_OK) return rc;
   b2d_ctx::OptimBucket ob;
   ob.nseg = nparam; ob.n = static_cast<size_t>(cur);
-  void *a = nullptr, *b = nullptr;
-  B2D_CUDA(ctx, cudaMalloc(&a, ptr.size() * sizeof(float*)));
-  B2D_CUDA(ctx, cudaMalloc(&b, start.size() * sizeof(unsigned)));
-  B2D_CUDA(ctx, cudaMemcpy(a, ptr.data(), ptr.size() * sizeof(float*), cudaMemcpyHostToDevice));
-  B2D_CUDA(ctx, cudaMemcpy(b, start.data(), start.size() * sizeof(unsigned), cudaMemcpyHostToDevice));
-  ob.d_ptr = static_cast<float**>(a); ob.d_start = static_cast<unsigned*>(b);
+  rc = upload_table(ctx, ptr, &ob.d_ptr);
+  if (rc == B2D_OK) rc = upload_table(ctx, start, &ob.d_start);
+  if (rc != B2D_OK) return rc;
   ctx->optim_buckets[bucket_id] = ob;
   return B2D_OK;
 }
@@ -1775,12 +1676,9 @@ int b2d_bucket_optim(b2d_ctx* ctx, int bucket_id, const float* grads, size_t n, 
   P.state1_ptr = it->second.d_ptr + it->second.nseg; P.state2_ptr = it->second.d_ptr + 2 * it->second.nseg;
   P.grads = grads; P.n = n; P.kind = kind;
   P.lr = hp->lr; P.momentum = momentum; P.weight_decay = hp->weight_decay;
-  if (kind == 1) fill_adam_consts(hp, &P.adam);
-  size_t grid = (n + kStThreads * 4 - 1) / (kStThreads * 4);
-  if (grid < 1) grid = 1;
-  const size_t cap = static_cast<size_t>(ctx->sm_count) * 2;
-  if (grid > cap) grid = cap;
-  bucket_optim_kernel<<<static_cast<int>(grid), kStThreads, 0, static_cast<cudaStream_t>(stream)>>>(P);
+  if (kind == 1) P.adam = adam_consts(*hp);
+  const int grid = clamp_grid(n, kStThreads * 4, static_cast<size_t>(ctx->sm_count) * 2);
+  bucket_optim_kernel<<<grid, kStThreads, 0, static_cast<cudaStream_t>(stream)>>>(P);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return fail(ctx, B2D_ERR_CUDA, "kernel launch failed: %s", cudaGetErrorString(e));
   ctx->launches += 1;
@@ -1921,7 +1819,6 @@ int b2d_ctx_stats(b2d_ctx* ctx, b2d_stats* out) {
   {
     DeviceGuard guard(ctx->device);
     resolve_timing(ctx, false);
-    resolve_exch_timing(ctx, false);
   }
   memset(out, 0, sizeof(*out));
   out->exch_launches = ctx->exch_launches; out->exch_timed = ctx->exch_timed; out->exch_ms = ctx->exch_ms;
@@ -1943,7 +1840,6 @@ int b2d_ctx_reset_stats(b2d_ctx* ctx) {
   {
     DeviceGuard guard(ctx->device);
     resolve_timing(ctx, true);
-    resolve_exch_timing(ctx, true);
   }
   ctx->launches = 0; ctx->timed_launches = 0; ctx->timed_ms = 0.0;
   ctx->exch_launches = 0; ctx->exch_timed = 0; ctx->exch_ms = 0.0;

@@ -1,0 +1,102 @@
+// b2d_launch.cuh — the host-side decisions around the kernel launches that b2d.cu and the CPU emulator
+// (emu/emu_harness.cpp) share: which specialisation of a kernel a world size runs, Adam's host constants, the chunk
+// geometry of the staged exchange and the owner-segment table of a reduce bucket.  Pure host code without CUDA
+// runtime calls, so that the emulated launches exercise the very decisions the library makes.
+#pragma once
+
+#include <math.h>
+
+#include <algorithm>
+#include <string>
+#include <type_traits>
+#include <vector>
+
+#include "b2d_kernels.cuh"
+
+namespace b2d {
+
+// The kernels that read peers are specialised for 2, 4 and 8 ranks; W = 0 is the generic build for any other world
+// size.  Calls f(std::integral_constant<int, W>{}) with the specialisation that `world` runs.
+template <typename F>
+void dispatch_world(int world, F&& f) {
+  switch (world) {
+    case 2: f(std::integral_constant<int, 2>{}); break;
+    case 4: f(std::integral_constant<int, 4>{}); break;
+    case 8: f(std::integral_constant<int, 8>{}); break;
+    default: f(std::integral_constant<int, 0>{}); break;
+  }
+}
+
+// Python-float (double) arithmetic of torch/optim/adam.py:503-541, cast once.
+inline AdamConsts adam_consts(const b2d_adam& adam) {
+  AdamConsts a{};
+  a.lr = adam.lr; a.beta1 = adam.beta1; a.beta2 = adam.beta2; a.eps = adam.eps; a.weight_decay = adam.weight_decay;
+  a.one_minus_beta1 = static_cast<float>(1.0 - static_cast<double>(adam.beta1));
+  a.one_minus_beta2 = static_cast<float>(1.0 - static_cast<double>(adam.beta2));
+  double b1p = 1.0, b2p = 1.0;
+  for (int i = 0; i < adam.step; ++i) { b1p *= static_cast<double>(adam.beta1); b2p *= static_cast<double>(adam.beta2); }
+  a.step_size = static_cast<float>(static_cast<double>(adam.lr) / (1.0 - b1p));
+  a.inv_bc2_sqrt = 1.0f / static_cast<float>(sqrt(1.0 - b2p));
+  a.decay_mul = static_cast<float>(1.0 - static_cast<double>(adam.lr) * static_cast<double>(adam.weight_decay));
+  a.adamw = adam.adamw;
+  return a;
+}
+
+// Chunk c of a staged exchange of n elements: npacks wire packs of epp elements, chunk_packs packs per chunk.
+struct ChunkSpan {
+  size_t p0;        // first pack of the chunk
+  size_t packs;     // packs in the chunk
+  size_t n;         // elements of the bucket in the chunk (S and U)
+  size_t n_valid;   // fp32 elements in the chunk when the bucket is exchanged in place (X; the last pack may be partial)
+};
+
+inline ChunkSpan chunk_span(int c, size_t npacks, size_t chunk_packs, size_t n, size_t epp) {
+  ChunkSpan s;
+  s.p0 = static_cast<size_t>(c) * chunk_packs;
+  s.packs = npacks - s.p0 < chunk_packs ? npacks - s.p0 : chunk_packs;
+  s.n = (s.p0 + s.packs) * epp <= n ? s.packs * epp : n - s.p0 * epp;
+  s.n_valid = n - s.p0 * 4 < s.packs * 4 ? n - s.p0 * 4 : s.packs * 4;
+  return s;
+}
+
+// The segment table of a reduce bucket (b2d_owner.cuh) in the order the owner kernels walk it.
+struct OwnerTable {
+  std::vector<long long> flat_off;         // flat offset of each merged segment
+  std::vector<unsigned> start;             // its first staging pack; one entry more, the bucket's total
+  unsigned owner_pack[B2D_MAX_WORLD + 1];  // staging packs [owner_pack[r], owner_pack[r+1]) belong to owner r
+};
+
+// Sorts the segments by (owner, offset) and merges runs that touch.  Returns an empty string, or why the segments
+// do not form a valid bucket.
+inline std::string build_owner_table(const b2d_seg* segs, int nseg, int world, int wire, OwnerTable* t) {
+  const long long epp = wire == B2D_WIRE_BF16 ? 8 : 4;
+  std::vector<b2d_seg> v(segs, segs + nseg);
+  for (const b2d_seg& sgm : v) {
+    if (sgm.owner < 0 || sgm.owner >= world) return "segment owner " + std::to_string(sgm.owner) + " out of range";
+    if (sgm.flat_off < 0 || sgm.len <= 0 || sgm.flat_off % 8 != 0 || sgm.len % 8 != 0)
+      return "segments must be non-empty, 8-element aligned runs (got " + std::to_string(sgm.flat_off) + " + " +
+             std::to_string(sgm.len) + ")";
+  }
+  std::stable_sort(v.begin(), v.end(), [](const b2d_seg& a, const b2d_seg& b) { return a.owner != b.owner ? a.owner < b.owner : a.flat_off < b.flat_off; });
+  std::vector<b2d_seg> m;
+  for (const b2d_seg& sgm : v) {
+    if (!m.empty() && m.back().owner == sgm.owner && m.back().flat_off + m.back().len == sgm.flat_off) m.back().len += sgm.len;
+    else m.push_back(sgm);
+  }
+  t->flat_off.assign(m.size(), 0);
+  t->start.assign(m.size() + 1, 0);
+  unsigned long long cum = 0;
+  int next_owner = 0;
+  for (size_t i = 0; i < m.size(); ++i) {
+    while (next_owner <= m[i].owner) t->owner_pack[next_owner++] = static_cast<unsigned>(cum);
+    t->flat_off[i] = m[i].flat_off;
+    t->start[i] = static_cast<unsigned>(cum);
+    cum += static_cast<unsigned long long>(m[i].len / epp);
+    if (cum > 0xffffffffull) return "reduce bucket too large";
+  }
+  t->start[m.size()] = static_cast<unsigned>(cum);
+  while (next_owner <= B2D_MAX_WORLD) t->owner_pack[next_owner++] = static_cast<unsigned>(cum);
+  return "";
+}
+
+}  // namespace b2d

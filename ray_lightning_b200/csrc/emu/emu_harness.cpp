@@ -15,6 +15,7 @@
 #include "../b2d_kernels.cuh"
 #include "../b2d_staged.cuh"
 #include "../b2d_owner.cuh"
+#include "../b2d_launch.cuh"
 
 thread_local EmuDim3 threadIdx, blockIdx, blockDim, gridDim;
 thread_local emu::Block* emu_block = nullptr;
@@ -100,15 +101,6 @@ void run_exch(const ExParams& P, bool bf16, bool nvls, bool inplace) {
   else if (bf16) { if (nvls) exch_kernel<W, true, true, false>(P); else exch_kernel<W, true, false, false>(P); }
   else { if (nvls) exch_kernel<W, false, true, false>(P); else exch_kernel<W, false, false, false>(P); }
 }
-void run_exch_w(int world, bool generic, const ExParams& P, bool bf16, bool nvls, bool inplace) {
-  if (generic) return run_exch<0>(P, bf16, nvls, inplace);
-  switch (world) {
-    case 2: return run_exch<2>(P, bf16, nvls, inplace);
-    case 4: return run_exch<4>(P, bf16, nvls, inplace);
-    case 8: return run_exch<8>(P, bf16, nvls, inplace);
-    default: return run_exch<0>(P, bf16, nvls, inplace);
-  }
-}
 
 }  // namespace
 
@@ -159,25 +151,27 @@ int emu_staged_allreduce(void* h, int nvls, int bf16, int inplace, float** bufs,
   auto S = [&](int r, int c) {
     StParams P{};
     P.scale = scale; P.rank = r; P.world = world; P.peers = peers;
-    const size_t p0 = static_cast<size_t>(c) * chunk_packs, pc = npacks - p0 < chunk_packs ? npacks - p0 : chunk_packs;
     if (inplace) {
       if (c != 0) return 0;
       P.epoch = epoch0 + nchunks - 1;
       return launch_one(1, 32, [P] { arrive_kernel(P); });
     }
-    P.grad = bufs[r] + p0 * epp;
-    P.n = (p0 + pc) * epp <= n ? pc * epp : n - p0 * epp;
-    P.wire = reinterpret_cast<uint4*>(g->arena[r] + wire_off) + p0;
+    const ChunkSpan cs = chunk_span(c, npacks, chunk_packs, n, epp);
+    P.grad = bufs[r] + cs.p0 * epp;
+    P.n = cs.n;
+    P.wire = reinterpret_cast<uint4*>(g->arena[r] + wire_off) + cs.p0;
     P.epoch = epoch0 + c;
     return bf16 ? launch_one(st_grid, kStThreads, [P] { stage_kernel<true>(P); }) : launch_one(st_grid, kStThreads, [P] { stage_kernel<false>(P); });
   };
   auto X = [&](int r, int c) {
     ExParams P{};
     P.scale = scale; P.rank = r; P.world = world; P.peers = peers; P.timeout_ns = 120ull * 1000000000ull; P.diag = nullptr;
-    const size_t p0 = static_cast<size_t>(c) * chunk_packs, pc = npacks - p0 < chunk_packs ? npacks - p0 : chunk_packs;
-    P.wire_off = wire_off + p0 * 16; P.npacks = pc; P.epoch = epoch0 + c;
-    P.n_valid = inplace ? (n - p0 * 4 < pc * 4 ? n - p0 * 4 : pc * 4) : 0;
-    return launch_one(ex_grid, kExThreads, [=] { run_exch_w(world, use_generic_w != 0, P, bf16 != 0, nvls != 0, inplace != 0); });
+    const ChunkSpan cs = chunk_span(c, npacks, chunk_packs, n, epp);
+    P.wire_off = wire_off + cs.p0 * 16; P.npacks = cs.packs; P.epoch = epoch0 + c;
+    P.n_valid = inplace ? cs.n_valid : 0;
+    return launch_one(ex_grid, kExThreads, [=] {
+      dispatch_world(use_generic_w ? 0 : world, [&](auto w) { run_exch<decltype(w)::value>(P, bf16 != 0, nvls != 0, inplace != 0); });
+    });
   };
   auto WU = [&](int r, int c) {
     ExParams P{};
@@ -186,10 +180,10 @@ int emu_staged_allreduce(void* h, int nvls, int bf16, int inplace, float** bufs,
     if (rc != 0 || inplace) return rc;
     StParams Q{};
     Q.scale = scale; Q.rank = r; Q.world = world; Q.peers = peers;
-    const size_t p0 = static_cast<size_t>(c) * chunk_packs, pc = npacks - p0 < chunk_packs ? npacks - p0 : chunk_packs;
-    Q.grad = bufs[r] + p0 * epp;
-    Q.n = (p0 + pc) * epp <= n ? pc * epp : n - p0 * epp;
-    Q.wire = reinterpret_cast<uint4*>(g->arena[r] + wire_off) + p0;
+    const ChunkSpan cs = chunk_span(c, npacks, chunk_packs, n, epp);
+    Q.grad = bufs[r] + cs.p0 * epp;
+    Q.n = cs.n;
+    Q.wire = reinterpret_cast<uint4*>(g->arena[r] + wire_off) + cs.p0;
     Q.epoch = epoch0 + c;
     return bf16 ? launch_one(st_grid, kStThreads, [Q] { unstage_kernel<true>(Q); }) : launch_one(st_grid, kStThreads, [Q] { unstage_kernel<false>(Q); });
   };
@@ -242,16 +236,11 @@ int emu_reduce_to_owner(void* h, int bf16, int nvls, float** grads, float** redu
   auto X = [&](int r) {
     const SegParams P = mk(r);
     auto run = [=] {
-      auto go = [&](auto w) {
+      dispatch_world(use_generic_w ? 0 : world, [&](auto w) {
         constexpr int W = decltype(w)::value;
         if (bf16) { if (nvls) seg_reduce_kernel<W, true, true>(P); else seg_reduce_kernel<W, true, false>(P); }
         else { if (nvls) seg_reduce_kernel<W, false, true>(P); else seg_reduce_kernel<W, false, false>(P); }
-      };
-      if (use_generic_w) go(std::integral_constant<int, 0>{});
-      else if (world == 2) go(std::integral_constant<int, 2>{});
-      else if (world == 4) go(std::integral_constant<int, 4>{});
-      else if (world == 8) go(std::integral_constant<int, 8>{});
-      else go(std::integral_constant<int, 0>{});
+      });
     };
     return launch_one(2, kExThreads, run);
   };
@@ -286,23 +275,13 @@ int emu_adam_push(void* h, int nvls, size_t param_off, float** m, float** v, flo
     P.lo = shard_off[r]; P.hi = shard_off[r + 1]; P.ngroups = ngroups;
     if (ngroups > 0) {
       P.group_lo[0] = glo[r]; P.group_hi[0] = ghi[r];
-      AdamConsts& a = P.group[0];
-      a.lr = lr; a.beta1 = beta1; a.beta2 = beta2; a.eps = eps; a.weight_decay = wd;
-      a.one_minus_beta1 = static_cast<float>(1.0 - static_cast<double>(beta1));
-      a.one_minus_beta2 = static_cast<float>(1.0 - static_cast<double>(beta2));
-      double b1p = 1.0, b2p = 1.0;
-      for (int i = 0; i < step; ++i) { b1p *= static_cast<double>(beta1); b2p *= static_cast<double>(beta2); }
-      a.step_size = static_cast<float>(static_cast<double>(lr) / (1.0 - b1p));
-      a.inv_bc2_sqrt = 1.0f / static_cast<float>(std::sqrt(1.0 - b2p));
-      a.decay_mul = static_cast<float>(1.0 - static_cast<double>(lr) * static_cast<double>(wd));
-      a.adamw = adamw;
+      P.group[0] = adam_consts(b2d_adam{lr, beta1, beta2, eps, wd, step, adamw, 0});
     }
     P.rank = r; P.world = world; P.epoch = epoch; P.peers = peers;
     auto run = [=] {
-      if (use_generic_w) { if (nvls) adam_push_kernel<0, true>(P); else adam_push_kernel<0, false>(P); }
-      else if (world == 2) { if (nvls) adam_push_kernel<2, true>(P); else adam_push_kernel<2, false>(P); }
-      else if (world == 4) { if (nvls) adam_push_kernel<4, true>(P); else adam_push_kernel<4, false>(P); }
-      else { if (nvls) adam_push_kernel<0, true>(P); else adam_push_kernel<0, false>(P); }
+      dispatch_world(use_generic_w ? 0 : world, [&](auto w) {
+        if (nvls) adam_push_kernel<decltype(w)::value, true>(P); else adam_push_kernel<decltype(w)::value, false>(P);
+      });
     };
     return launch_one(2, kExThreads, run);
   };
@@ -329,18 +308,7 @@ int emu_bucket_optim(float** params, float** state1, float** state2, const unsig
   OptimParams P{};
   P.param_ptr = params; P.state1_ptr = state1; P.state2_ptr = state2; P.seg_start = seg_start; P.nseg = nseg;
   P.grads = grads; P.n = n; P.kind = kind; P.lr = lr; P.momentum = momentum; P.weight_decay = wd;
-  if (kind == 1) {
-    AdamConsts& a = P.adam;
-    a.lr = lr; a.beta1 = beta1; a.beta2 = beta2; a.eps = eps; a.weight_decay = wd;
-    a.one_minus_beta1 = static_cast<float>(1.0 - static_cast<double>(beta1));
-    a.one_minus_beta2 = static_cast<float>(1.0 - static_cast<double>(beta2));
-    double b1p = 1.0, b2p = 1.0;
-    for (int i = 0; i < step; ++i) { b1p *= static_cast<double>(beta1); b2p *= static_cast<double>(beta2); }
-    a.step_size = static_cast<float>(static_cast<double>(lr) / (1.0 - b1p));
-    a.inv_bc2_sqrt = 1.0f / static_cast<float>(std::sqrt(1.0 - b2p));
-    a.decay_mul = static_cast<float>(1.0 - static_cast<double>(lr) * static_cast<double>(wd));
-    a.adamw = adamw;
-  }
+  if (kind == 1) P.adam = adam_consts(b2d_adam{lr, beta1, beta2, eps, wd, step, adamw, 0});
   return launch_one(2, kStThreads, [P] { bucket_optim_kernel(P); });
 }
 
@@ -365,20 +333,11 @@ int emu_allreduce(void* h, int algo, int bf16, float** bufs, size_t n, float sca
     P.rank = r; P.world = world; P.timeout_ns = 60ull * 1000000000ull; P.diag = nullptr; P.peers = make_peers(*g);
     params[r] = P;
     const ArParams* pp = &params[r];
-    if (use_generic_w) {
-      bodies[r] = bf16 ? std::function<void()>([=] { run_ar<0, true>(algo, *pp, pipe_k); })
-                       : std::function<void()>([=] { run_ar<0, false>(algo, *pp, pipe_k); });
-    } else {
-      switch (world) {
-        case 2: bodies[r] = bf16 ? std::function<void()>([=] { run_ar<2, true>(algo, *pp, pipe_k); })
-                                 : std::function<void()>([=] { run_ar<2, false>(algo, *pp, pipe_k); }); break;
-        case 4: bodies[r] = bf16 ? std::function<void()>([=] { run_ar<4, true>(algo, *pp, pipe_k); })
-                                 : std::function<void()>([=] { run_ar<4, false>(algo, *pp, pipe_k); }); break;
-        case 8: bodies[r] = bf16 ? std::function<void()>([=] { run_ar<8, true>(algo, *pp, pipe_k); })
-                                 : std::function<void()>([=] { run_ar<8, false>(algo, *pp, pipe_k); }); break;
-        default: return -1;
-      }
-    }
+    dispatch_world(use_generic_w ? 0 : world, [&](auto w) {
+      constexpr int W = decltype(w)::value;
+      bodies[r] = bf16 ? std::function<void()>([=] { run_ar<W, true>(algo, *pp, pipe_k); })
+                       : std::function<void()>([=] { run_ar<W, false>(algo, *pp, pipe_k); });
+    });
   }
   return launch_all(world, grid, kThreads, bodies);
 }
@@ -411,25 +370,15 @@ int emu_sharded_step(void* h, int bf16, float** grads, size_t param_off, float**
     for (int i = world + 1; i <= B2D_MAX_WORLD; ++i) P.off[i] = shard_off[world];
     P.stage_off = stage_base + (parity & 1) * half; P.scale = scale; P.rank = r; P.world = world;
     P.do_stage_reduce = 1; P.do_adam = 1; P.do_gather = 1; P.end_barrier = 0;
-    AdamConsts& a = P.adam;   // same host arithmetic as sharded_common() in b2d.cu
-    a.lr = lr; a.beta1 = beta1; a.beta2 = beta2; a.eps = eps; a.weight_decay = wd;
-    a.one_minus_beta1 = static_cast<float>(1.0 - static_cast<double>(beta1));
-    a.one_minus_beta2 = static_cast<float>(1.0 - static_cast<double>(beta2));
-    double b1p = 1.0, b2p = 1.0;
-    for (int i = 0; i < step; ++i) { b1p *= static_cast<double>(beta1); b2p *= static_cast<double>(beta2); }
-    a.step_size = static_cast<float>(static_cast<double>(lr) / (1.0 - b1p));
-    a.inv_bc2_sqrt = 1.0f / static_cast<float>(std::sqrt(1.0 - b2p));
-    a.decay_mul = static_cast<float>(1.0 - static_cast<double>(lr) * static_cast<double>(wd));
-    a.adamw = adamw;
+    P.adam = adam_consts(b2d_adam{lr, beta1, beta2, eps, wd, step, adamw, 0});
     P.timeout_ns = 60ull * 1000000000ull; P.diag = nullptr; P.peers = make_peers(*g);
     params[r] = P;
     const ShParams* pp = &params[r];
-    auto mk = [&](auto fn) { return std::function<void()>([=] { fn(*pp); }); };
-    if (use_generic_w) bodies[r] = bf16 ? mk(k456_sharded_kernel<0, true>) : mk(k456_sharded_kernel<0, false>);
-    else if (world == 2) bodies[r] = bf16 ? mk(k456_sharded_kernel<2, true>) : mk(k456_sharded_kernel<2, false>);
-    else if (world == 4) bodies[r] = bf16 ? mk(k456_sharded_kernel<4, true>) : mk(k456_sharded_kernel<4, false>);
-    else if (world == 8) bodies[r] = bf16 ? mk(k456_sharded_kernel<8, true>) : mk(k456_sharded_kernel<8, false>);
-    else return -1;
+    dispatch_world(use_generic_w ? 0 : world, [&](auto w) {
+      constexpr int W = decltype(w)::value;
+      bodies[r] = bf16 ? std::function<void()>([=] { k456_sharded_kernel<W, true>(*pp); })
+                       : std::function<void()>([=] { k456_sharded_kernel<W, false>(*pp); });
+    });
   }
   return launch_all(world, grid, kThreads, bodies);
 }
@@ -476,6 +425,19 @@ int emu_allgather(void* h, size_t buf_off, size_t n, const long long* shard_off,
     bodies[r] = std::function<void()>([=] { k456_sharded_kernel<0, false>(*pp); });
   }
   return launch_all(world, grid, kThreads, bodies);
+}
+
+// b2d_bucket_register's table for segments given as (flat_off, len, owner) triples: fills flat_off[nseg], start[nseg + 1]
+// and owner_pack[world + 1].  Returns the number of merged segments, or -1 if the segments are rejected.
+int emu_owner_table(const long long* segs, int nseg, int world, int bf16, long long* flat_off, unsigned* start, unsigned* owner_pack) {
+  std::vector<b2d_seg> v(nseg);
+  for (int i = 0; i < nseg; ++i) v[i] = b2d_seg{segs[3 * i], segs[3 * i + 1], static_cast<int32_t>(segs[3 * i + 2]), 0};
+  OwnerTable t;
+  if (!build_owner_table(v.data(), nseg, world, bf16 ? B2D_WIRE_BF16 : B2D_WIRE_FP32, &t).empty()) return -1;
+  std::copy(t.flat_off.begin(), t.flat_off.end(), flat_off);
+  std::copy(t.start.begin(), t.start.end(), start);
+  std::copy(t.owner_pack, t.owner_pack + world + 1, owner_pack);
+  return static_cast<int>(t.flat_off.size());
 }
 
 float* emu_arena_ptr(void* h, int rank, size_t off) {

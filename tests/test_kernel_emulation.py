@@ -54,6 +54,7 @@ def emu(tmp_path_factory):
     lib.emu_reduce_scatter.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.POINTER(FP), ctypes.POINTER(FP), ctypes.c_size_t,
                                        ctypes.POINTER(ctypes.c_longlong), ctypes.c_float, ctypes.c_size_t, ctypes.c_int, ctypes.c_int]
     lib.emu_allgather.argtypes = [ctypes.c_void_p, ctypes.c_size_t, ctypes.c_size_t, ctypes.POINTER(ctypes.c_longlong), ctypes.c_int]
+    lib.emu_owner_table.argtypes = [LP, ctypes.c_int, ctypes.c_int, ctypes.c_int, LP, UP, UP]
     lib.emu_arena_ptr.restype = FP
     lib.emu_arena_ptr.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_size_t]
     return lib
@@ -282,28 +283,16 @@ def test_reduce_scatter_and_allgather_alone_on_cpu_threads(emu, world):
         emu.emu_group_destroy(g)
 
 
-def _seg_table(segs, world, epp):
-    """What b2d_bucket_register builds: segments sorted by (owner, offset), touching runs merged, cumulative pack starts."""
-    segs = sorted(segs, key=lambda s: (s[2], s[0]))
-    merged = []
-    for off, n, owner in segs:
-        if merged and merged[-1][2] == owner and merged[-1][0] + merged[-1][1] == off:
-            merged[-1][1] += n
-        else:
-            merged.append([off, n, owner])
-    flat, start, owner_pack, cum, nxt = [], [], [], 0, 0
-    for off, n, owner in merged:
-        while nxt <= owner:
-            owner_pack.append(cum)
-            nxt += 1
-        flat.append(off)
-        start.append(cum)
-        cum += n // epp
-    start.append(cum)
-    while nxt <= world:
-        owner_pack.append(cum)
-        nxt += 1
-    return flat, start, owner_pack
+def _seg_table(emu, segs, world, epp):
+    """What b2d_bucket_register builds (segments sorted by (owner, offset), touching runs merged, cumulative pack starts),
+    from the library's own table builder."""
+    flat = (ctypes.c_longlong * len(segs))()
+    start = (ctypes.c_uint * (len(segs) + 1))()
+    owner_pack = (ctypes.c_uint * (world + 1))()
+    triples = (ctypes.c_longlong * (3 * len(segs)))(*[x for seg in segs for x in seg])
+    nseg = emu.emu_owner_table(triples, len(segs), world, int(epp == 8), flat, start, owner_pack)
+    assert nseg > 0
+    return list(flat[:nseg]), list(start[:nseg + 1]), list(owner_pack)
 
 
 @pytest.mark.parametrize("world,generic", [(2, 0), (4, 0), (3, 1)])
@@ -336,7 +325,7 @@ def test_reduce_to_owner_and_adam_push_on_cpu_threads(emu, world, generic, bf16,
             grads = [t.numpy().copy() for t in per_rank]
             wire_off = sig + (1 << 20)
             for b, segs in enumerate(buckets):
-                flat, start, opack = _seg_table(segs, world, epp)
+                flat, start, opack = _seg_table(emu, segs, world, epp)
                 rc = emu.emu_reduce_to_owner(g, bf16, nvls, ptrs(grads), ptrs(reduced), off, (ctypes.c_longlong * len(flat))(*flat),
                                              (ctypes.c_uint * len(start))(*start), len(flat), (ctypes.c_uint * len(opack))(*opack),
                                              wire_off, scale, 1, rep, epoch, (rep + b) % 2, generic)
@@ -447,7 +436,7 @@ def test_owner_path_with_ranks_that_own_nothing(emu):
         offs = [o for _, o in sorted(offs)]
         total = cur
         segs = [(offs[i], numels[i], owner[i]) for i in range(3)]
-        flat, start, opack = _seg_table(segs, world, 4)
+        flat, start, opack = _seg_table(emu, segs, world, 4)
         assert opack[2] == opack[3]                      # rank 2's range of the staging region is empty
         per_rank = [torch.randn(total, generator=torch.Generator().manual_seed(r)) * 0.1 for r in range(world)]
         grads = [t.numpy().copy() for t in per_rank]
