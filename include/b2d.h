@@ -286,6 +286,33 @@ int b2d_bucket_optim(b2d_ctx* ctx, int bucket_id, const float* grads, size_t n, 
  * All-ranks barrier enqueued on `stream` (also quiesces the arena before slots are re-laid out). */
 int b2d_barrier(b2d_ctx* ctx, void* stream);
 
+/* ---- synchronised BatchNorm (b2d_syncbn.cuh) ---------------------------------------------- */
+
+/* Declare BatchNorm layer `layer_id` with `channels` channels: takes its exchange region (two generations of
+ * W forward rows and two of W backward rows, about 32 x W x channels bytes) from the arena and writes the region's
+ * arena offset to *offset (may be NULL).  Every rank must register the same layers in the same order, so that the
+ * offsets agree; registering a layer again with the same channel count is a no-op.  Host only. */
+int b2d_bn_register(b2d_ctx* ctx, int layer_id, int channels, size_t* offset);
+
+/* Replaces: torch.nn.SyncBatchNorm's forward statistics exchange (torch/nn/modules/_functions.py:65-115: cat,
+ * all_gather_into_tensor, the host-side mask of empty ranks, batch_norm_gather_stats_with_counts).
+ * mean / invstd: this rank's batch_norm_stats (fp32 [C]); count: its elements per channel.  A rank with count == 0
+ * passes NULL mean / invstd and pushes a zero row.  Writes the statistics of the whole batch over every rank with
+ * count > 0 (rank-ordered merge, fp32) to mean_out / invstd_out (fp32 [C]), every rank's count to counts_out
+ * (int32 [W], zeros kept) and, when non-NULL, updates running_mean / running_var (fp32 [C]) in place with
+ * `momentum` and the unbiased variance.  Enqueued on `stream`; no host synchronisation.
+ * phases: bit 0 push, bit 1 wait + combine (3 = both); hosts that drive several ranks from one thread issue bit 0 for
+ * every rank, then bit 1. */
+int b2d_bn_stats_exchange(b2d_ctx* ctx, int layer_id, const float* mean, const float* invstd, float count,
+                          float eps, float momentum, float* mean_out, float* invstd_out, int32_t* counts_out,
+                          float* running_mean, float* running_var, unsigned phases, void* stream);
+
+/* Replaces: torch.nn.SyncBatchNorm's backward exchange (torch/nn/modules/_functions.py:155-165: cat, all_reduce
+ * SUM, split).  sum_dy / sum_dy_xmu: this rank's batch_norm_backward_reduce outputs (fp32 [C]; NULL: zeros).
+ * Writes their rank-ordered fp32 sums over every rank to sum_dy_out / sum_dy_xmu_out.  phases as above. */
+int b2d_bn_grad_exchange(b2d_ctx* ctx, int layer_id, const float* sum_dy, const float* sum_dy_xmu,
+                         float* sum_dy_out, float* sum_dy_xmu_out, unsigned phases, void* stream);
+
 /* ---- symmetric arena ------------------------------------------------------------------- */
 
 /* Bump-allocate `bytes` (256-byte aligned) of caller-visible symmetric memory.  Every rank

@@ -34,7 +34,7 @@ EXPORTED_SYMBOLS = [
     "b2d_allreduce_bucket_phased", "b2d_ctx_set_chunk_bytes", "b2d_ctx_set_exch_ctas", "b2d_ctx_set_nvls_auto",
     "b2d_peer_bw", "b2d_pool_bind", "b2d_pool_alloc", "b2d_pool_free", "b2d_ctx_set_inplace",
     "b2d_bucket_register", "b2d_reduce_to_owner", "b2d_adam_push", "b2d_ctx_set_auto_profile",
-    "b2d_optim_register", "b2d_bucket_optim",
+    "b2d_optim_register", "b2d_bucket_optim", "b2d_bn_register", "b2d_bn_stats_exchange", "b2d_bn_grad_exchange",
 ]
 PROFILE_OVERLAP, PROFILE_LATENCY = 0, 1
 RTO_ZERO_GRADS, RTO_ACCUMULATE, RTO_NVLS = 1, 2, 4
@@ -122,6 +122,9 @@ def _declare(lib):
                              c.POINTER(AdamParams), vp, vp],
         "b2d_reduce_scatter": [vp, c.c_int, vp, vp, sz, c.POINTER(c.c_int64), c.c_int, c.c_float, vp, vp],
         "b2d_allgather": [vp, vp, sz, c.POINTER(c.c_int64), vp, vp],
+        "b2d_bn_register": [vp, c.c_int, c.c_int, c.POINTER(sz)],
+        "b2d_bn_stats_exchange": [vp, c.c_int, vp, vp, c.c_float, c.c_float, c.c_float, vp, vp, vp, vp, vp, c.c_uint, vp],
+        "b2d_bn_grad_exchange": [vp, c.c_int, vp, vp, vp, vp, c.c_uint, vp],
         "b2d_barrier": [vp, vp],
         "b2d_arena_alloc": [vp, sz, c.POINTER(vp), c.POINTER(sz)],
         "b2d_arena_reset": [vp],
@@ -345,6 +348,26 @@ class Context:
     def bucket_optim(self, bucket_id, grads_ptr, n, kind, hp, momentum, stream):
         self._check(self._lib.b2d_bucket_optim(self._ctx, int(bucket_id), ctypes.c_void_p(grads_ptr), int(n), int(kind),
                                                ctypes.byref(hp), float(momentum), _stream_ptr(stream)))
+
+    def bn_register(self, layer_id, channels):
+        """Returns the arena offset of the layer's exchange region."""
+        off = ctypes.c_size_t()
+        self._check(self._lib.b2d_bn_register(self._ctx, int(layer_id), int(channels), ctypes.byref(off)))
+        return off.value
+
+    def bn_stats_exchange(self, layer_id, mean_ptr, invstd_ptr, count, eps, momentum, mean_out_ptr, invstd_out_ptr,
+                          counts_out_ptr, running_mean_ptr, running_var_ptr, phases, stream):
+        vp = ctypes.c_void_p
+        self._check(self._lib.b2d_bn_stats_exchange(
+            self._ctx, int(layer_id), vp(mean_ptr), vp(invstd_ptr), float(count), float(eps), float(momentum),
+            vp(mean_out_ptr), vp(invstd_out_ptr), vp(counts_out_ptr), vp(running_mean_ptr), vp(running_var_ptr),
+            int(phases), _stream_ptr(stream)))
+
+    def bn_grad_exchange(self, layer_id, sum_dy_ptr, sum_dy_xmu_ptr, sum_dy_out_ptr, sum_dy_xmu_out_ptr, phases, stream):
+        vp = ctypes.c_void_p
+        self._check(self._lib.b2d_bn_grad_exchange(self._ctx, int(layer_id), vp(sum_dy_ptr), vp(sum_dy_xmu_ptr),
+                                                   vp(sum_dy_out_ptr), vp(sum_dy_xmu_out_ptr), int(phases),
+                                                   _stream_ptr(stream)))
 
     def barrier(self, stream):
         self._check(self._lib.b2d_barrier(self._ctx, _stream_ptr(stream)))

@@ -433,8 +433,14 @@ class DDPSpawnStrategy(ParallelStrategy):
                 hook = self._ddp_comm_wrapper(hook)
             self.model.register_comm_hook(self._ddp_comm_state, hook)
 
+    def configure_sync_batchnorm(self, model):
+        return torch.nn.SyncBatchNorm.convert_sync_batchnorm(model)
+
     def setup(self, trainer):
         self.model_to_device()
+        # PL 1.6 order: convert after moving the model, before wrapping it
+        if getattr(self, "sync_batchnorm", False):
+            self.model = self.configure_sync_batchnorm(self.model)
         if trainer.state.fn == TrainerFn.FITTING:
             self.configure_ddp()
             self.setup_optimizers(trainer)
@@ -520,7 +526,7 @@ class Trainer:
                  limit_train_batches=1.0, limit_val_batches=1.0, limit_test_batches=1.0, enable_progress_bar=False,
                  checkpoint_callback=None, enable_checkpointing=True, precision=32, num_sanity_val_steps=0,
                  resume_from_checkpoint=None, reload_dataloaders_every_n_epochs=0, gpus=None, logger=None,
-                 progress_bar_refresh_rate=None, log_every_n_steps=50, **_ignored):
+                 progress_bar_refresh_rate=None, log_every_n_steps=50, sync_batchnorm=False, **_ignored):
         self.default_root_dir = str(default_root_dir) if default_root_dir is not None else os.getcwd()
         self.callbacks = list(callbacks or [])
         if checkpoint_callback is not None:
@@ -529,6 +535,7 @@ class Trainer:
             self.callbacks.append(ModelCheckpoint())
         self.strategy = strategy if strategy is not None else Strategy()
         self.strategy.precision = precision
+        self.strategy.sync_batchnorm = bool(sync_batchnorm)
         self.max_epochs, self.max_steps = max_epochs, max_steps
         self.limit_train_batches, self.limit_val_batches, self.limit_test_batches = \
             limit_train_batches, limit_val_batches, limit_test_batches

@@ -202,6 +202,54 @@ class _Base:
         self.ctx.allgather(buf.data_ptr(), buf.numel(), shard_off, ws, cs)
         return buf
 
+    # ---- synchronised BatchNorm (b2d_syncbn.cuh) -------------------------------------------------------------
+    def bn_register(self, layer_id, channels):
+        """Give BatchNorm layer ``layer_id`` its exchange region in the arena; returns the region's arena offset.
+        Every rank registers the same layers in the same order."""
+        off = self.ctx.bn_register(layer_id, channels)
+        if getattr(self, "_bn_channels", None) is None:
+            self._bn_channels = {}
+        self._bn_channels[layer_id] = int(channels)
+        return off
+
+    def bn_register_all(self, layers):
+        """``layers``: [(layer_id, channels)]; returns their arena offsets."""
+        return [self.bn_register(i, c) for i, c in layers]
+
+    def _bn_check(self, layer_id, tensors, dtype=torch.float32):
+        c = (getattr(self, "_bn_channels", None) or {}).get(layer_id)
+        if c is None:
+            raise ValueError("BatchNorm layer %d has not been registered (bn_register)" % layer_id)
+        for t in tensors:
+            if t is None:
+                continue
+            if not t.is_cuda or t.device.index != self.device_index:
+                raise ValueError("tensor is on %s, communicator on cuda:%d" % (t.device, self.device_index))
+            if t.dtype != dtype or not t.is_contiguous() or t.numel() != c:
+                raise ValueError("expected a contiguous %s tensor of %d elements, got %s %s" % (dtype, c, t.dtype, tuple(t.shape)))
+
+    def bn_stats_exchange(self, layer_id, mean, invstd, count, eps, momentum, mean_out, invstd_out, counts_out,
+                          running_mean=None, running_var=None, stream=None, phases=3):
+        """Synchronised BatchNorm statistics (b2d_bn_stats_exchange): this rank's ``mean`` / ``invstd`` over ``count``
+        elements per channel (None and 0 for an empty rank) -> the whole batch's ``mean_out`` / ``invstd_out``, every
+        rank's count in ``counts_out`` (int32 [W]) and the running statistics updated in place.  On ``stream``
+        (default: the current one), without host synchronisation."""
+        self._bn_check(layer_id, (mean, invstd, mean_out, invstd_out, running_mean, running_var))
+        if counts_out.dtype != torch.int32 or counts_out.numel() != self.world or not counts_out.is_cuda:
+            raise ValueError("counts_out must be a CUDA int32 tensor of %d elements" % self.world)
+        st = torch.cuda.current_stream(mean_out.device) if stream is None else stream
+        ptr = lambda t: 0 if t is None else t.data_ptr()
+        self.ctx.bn_stats_exchange(layer_id, ptr(mean), ptr(invstd), count, eps, momentum, ptr(mean_out), ptr(invstd_out),
+                                   ptr(counts_out), ptr(running_mean), ptr(running_var), phases, st)
+
+    def bn_grad_exchange(self, layer_id, sum_dy, sum_dy_xmu, sum_dy_out, sum_dy_xmu_out, stream=None, phases=3):
+        """Rank-ordered fp32 sums of every rank's ``sum_dy`` / ``sum_dy_xmu`` (None: zeros) into the outputs
+        (b2d_bn_grad_exchange)."""
+        self._bn_check(layer_id, (sum_dy, sum_dy_xmu, sum_dy_out, sum_dy_xmu_out))
+        st = torch.cuda.current_stream(sum_dy_out.device) if stream is None else stream
+        ptr = lambda t: 0 if t is None else t.data_ptr()
+        self.ctx.bn_grad_exchange(layer_id, ptr(sum_dy), ptr(sum_dy_xmu), ptr(sum_dy_out), ptr(sum_dy_xmu_out), phases, st)
+
     def arena_tensor(self, numel, dtype=torch.float32):
         t, _ = arena_tensor(self.ctx, numel, dtype, torch.device("cuda", self.device_index))
         return t
@@ -331,6 +379,18 @@ class Communicator(_Base):
         if required and not self.nvls:
             raise RuntimeError("NVLS multicast setup failed: %s" % err)
 
+    def bn_register_all(self, layers):
+        """Collective: register ``layers`` ([(layer_id, channels)], the same list in the same order on every rank) and
+        check over the control plane that every rank placed them at the same arena offsets."""
+        offs = super().bn_register_all(layers)
+        if self.world > 1 and dist.is_initialized():
+            allv = [None] * self.world
+            dist.all_gather_object(allv, offs, group=self.group)
+            if any(v != offs for v in allv):
+                raise RuntimeError("SyncBatchNorm regions landed at different arena offsets on different ranks: every "
+                                   "rank must register the same layers in the same order")
+        return offs
+
     def close(self):
         if self.ctx is not None:
             if self.world > 1 and dist.is_initialized():
@@ -437,6 +497,32 @@ class LoopbackGroup:
         for r, rk in enumerate(self.ranks):
             rk.allgather_(bufs[r], shard_off, wait_stream=torch.cuda.current_stream(bufs[r].device),
                           comm_stream=rk.stream)
+
+    def bn_register(self, layer_id, channels):
+        offs = [rk.bn_register(layer_id, channels) for rk in self.ranks]
+        if len(set(offs)) != 1:
+            raise RuntimeError("SyncBatchNorm region of layer %d at different arena offsets: %s" % (layer_id, offs))
+        return offs[0]
+
+    def bn_stats_exchange(self, layer_id, means, invstds, counts, eps, momentum, mean_outs, invstd_outs, counts_outs,
+                          running_means=None, running_vars=None):
+        """Rank r's arguments are the r-th entries.  Phase-major on the ranks' own streams (after the current stream):
+        push everywhere, then combine everywhere."""
+        for ph in (1, 2):
+            for r, rk in enumerate(self.ranks):
+                if ph == 1:
+                    rk.stream.wait_stream(torch.cuda.current_stream(torch.device("cuda", rk.device_index)))
+                rk.bn_stats_exchange(layer_id, means[r], invstds[r], counts[r], eps, momentum, mean_outs[r], invstd_outs[r],
+                                     counts_outs[r], None if running_means is None else running_means[r],
+                                     None if running_vars is None else running_vars[r], stream=rk.stream, phases=ph)
+
+    def bn_grad_exchange(self, layer_id, sum_dys, sum_dy_xmus, sum_dy_outs, sum_dy_xmu_outs):
+        for ph in (1, 2):
+            for r, rk in enumerate(self.ranks):
+                if ph == 1:
+                    rk.stream.wait_stream(torch.cuda.current_stream(torch.device("cuda", rk.device_index)))
+                rk.bn_grad_exchange(layer_id, sum_dys[r], sum_dy_xmus[r], sum_dy_outs[r], sum_dy_xmu_outs[r],
+                                    stream=rk.stream, phases=ph)
 
     def synchronize(self):
         for rk in self.ranks:

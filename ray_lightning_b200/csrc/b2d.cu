@@ -21,6 +21,7 @@
 #include "b2d_tma.cuh"
 #include "b2d_staged.cuh"
 #include "b2d_owner.cuh"
+#include "b2d_syncbn.cuh"
 #include "b2d_launch.cuh"
 
 using namespace b2d;
@@ -226,6 +227,19 @@ struct b2d_ctx {
   uint32_t push_epoch = 0;
   struct OptimBucket { int nseg = 0; size_t n = 0; float** d_ptr = nullptr; unsigned* d_start = nullptr; };   // d_ptr: [3][nseg] params | state1 | state2
   std::map<int, OptimBucket> optim_buckets;
+
+  // synchronised BatchNorm (b2d_syncbn.cuh): one arena region per registered layer, laid out as
+  // [forward gen 0 | forward gen 1 | backward gen 0 | backward gen 1], each generation W rows.  Index d: 0 forward,
+  // 1 backward.  op_epoch[d] != 0 while a pushed exchange waits for its combine phase.
+  struct BnLayer {
+    int channels = 0;
+    size_t off = 0;
+    unsigned calls[2] = {0, 0};
+    unsigned op_gen[2] = {0, 0};
+    uint32_t op_epoch[2] = {0, 0};
+  };
+  std::map<int, BnLayer> bn_layers;
+  uint32_t bn_epoch = 0;   // the BN exchanges' own epoch (Signal::bn), independent of the bucket exchanges' `epoch`
 
   unsigned long long* trace_dev = nullptr;   // debug: per-block phase stamps of the LAST allreduce launch
   int trace_grid = 0;
@@ -671,6 +685,7 @@ void preload_kernels() {
   preload_one(seg_stage_kernel<true>); preload_one(seg_stage_kernel<false>);
   for (int world : worlds) dispatch_world(world, preload_owner);
   preload_one(bucket_optim_kernel);
+  preload_one(bn_push_kernel); preload_one(bn_combine_kernel<true>); preload_one(bn_combine_kernel<false>);
   preload_one(k0_cast_scale_kernel<true>);
   preload_one(k0_cast_scale_kernel<false>);
   preload_one(barrier_kernel);
@@ -1694,6 +1709,100 @@ int b2d_barrier(b2d_ctx* ctx, void* stream) {
   return launch_barrier(ctx, static_cast<cudaStream_t>(stream));
 }
 
+// ---- synchronised BatchNorm (b2d_syncbn.cuh) -----------------------------------------------
+int b2d_bn_register(b2d_ctx* ctx, int layer_id, int channels, size_t* offset) {
+  if (ctx == nullptr) return fail(nullptr, B2D_ERR_INVALID, "ctx is NULL");
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  if (channels < 1) return fail(ctx, B2D_ERR_INVALID, "a BatchNorm layer needs at least one channel (got %d)", channels);
+  auto it = ctx->bn_layers.find(layer_id);
+  if (it != ctx->bn_layers.end()) {
+    if (it->second.channels != channels)
+      return fail(ctx, B2D_ERR_INVALID, "BatchNorm layer %d is registered with %d channels, not %d", layer_id, it->second.channels, channels);
+  } else {
+    const size_t W = static_cast<size_t>(ctx->world);
+    const size_t bytes = round_up(2 * W * (bn_fwd_row(channels) + bn_bwd_row(channels)) * 4, kAlign);
+    size_t off = 0;
+    if (!slot_region_alloc(ctx, bytes, &off))
+      return fail(ctx, B2D_ERR_NOMEM, "symmetric arena exhausted: BatchNorm layer %d needs %zu bytes, %zu free of %zu", layer_id,
+                  bytes, ctx->user_bottom - ctx->slot_top, ctx->arena_bytes);
+    b2d_ctx::BnLayer L;
+    L.channels = channels;
+    L.off = off;
+    it = ctx->bn_layers.emplace(layer_id, L).first;
+  }
+  if (offset != nullptr) *offset = it->second.off;
+  return B2D_OK;
+}
+
+// One BN exchange: K15 (phase bit 0) and K16 / K17 (bit 1) on `stream`.  a / b: this rank's two halves of the row.
+static int bn_exchange(b2d_ctx* ctx, int layer_id, bool fwd, const float* a, const float* b, float count, float eps,
+                       float momentum, float* out_a, float* out_b, int32_t* counts, float* running_mean, float* running_var,
+                       unsigned phases, void* stream) {
+  int rc = check_ready(ctx);
+  if (rc != B2D_OK) return rc;
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  auto it = ctx->bn_layers.find(layer_id);
+  if (it == ctx->bn_layers.end()) return fail(ctx, B2D_ERR_STATE, "BatchNorm layer %d has not been registered", layer_id);
+  if ((phases & 3u) == 0 || phases > 3u) return fail(ctx, B2D_ERR_INVALID, "bad phase mask %u (bit 0 push, bit 1 combine)", phases);
+  if ((phases & 1u) && fwd && !(count >= 0.f)) return fail(ctx, B2D_ERR_INVALID, "count must be >= 0");
+  if ((phases & 1u) && fwd && count > 0.f && (a == nullptr || b == nullptr))
+    return fail(ctx, B2D_ERR_INVALID, "a rank with count > 0 must pass its mean and invstd");
+  if ((phases & 2u) && (out_a == nullptr || out_b == nullptr || (fwd && counts == nullptr)))
+    return fail(ctx, B2D_ERR_INVALID, "NULL output");
+  b2d_ctx::BnLayer& L = it->second;
+  const int d = fwd ? 0 : 1;
+  if ((phases & 1u) && L.op_epoch[d] != 0)
+    return fail(ctx, B2D_ERR_STATE, "BatchNorm layer %d: push issued again before the previous exchange was combined", layer_id);
+  if (!(phases & 1u) && L.op_epoch[d] == 0)
+    return fail(ctx, B2D_ERR_STATE, "BatchNorm layer %d: combine issued before the push", layer_id);
+  DeviceGuard guard(ctx->device);
+  if (!guard.ok) return fail(ctx, B2D_ERR_CUDA, "cudaSetDevice(%d) failed", ctx->device);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const int C = L.channels;
+  const size_t W = static_cast<size_t>(ctx->world);
+  const size_t gen_bytes = W * (fwd ? bn_fwd_row(C) : bn_bwd_row(C)) * 4;
+  const size_t base = L.off + (fwd ? 0 : 2 * W * bn_fwd_row(C) * 4);
+  if (phases & 1u) {
+    L.op_gen[d] = L.calls[d]++ & 1u;
+    L.op_epoch[d] = ++ctx->bn_epoch;
+    BnPushParams P{};
+    P.a = a; P.b = b; P.count = fwd ? count : 0.f; P.channels = C; P.fwd = fwd ? 1 : 0;
+    P.region_off = base + L.op_gen[d] * gen_bytes;
+    P.rank = ctx->rank; P.world = ctx->world; P.epoch = L.op_epoch[d]; P.peers = ctx->peers;
+    bn_push_kernel<<<1, kBnThreads, 0, st>>>(P);
+    ctx->launches += 1;
+  }
+  if (phases & 2u) {
+    BnCombineParams P{};
+    P.region_off = base + L.op_gen[d] * gen_bytes;
+    P.channels = C; P.eps = eps; P.momentum = momentum;
+    P.out_a = out_a; P.out_b = out_b; P.counts = counts;
+    P.running_mean = fwd ? running_mean : nullptr; P.running_var = fwd ? running_var : nullptr;
+    set_peer_wait(ctx, &P);
+    P.epoch = L.op_epoch[d];
+    const int grid = clamp_grid(static_cast<size_t>(C), kBnThreads, static_cast<size_t>(ctx->sm_count));
+    if (fwd) bn_combine_kernel<true><<<grid, kBnThreads, 0, st>>>(P); else bn_combine_kernel<false><<<grid, kBnThreads, 0, st>>>(P);
+    ctx->launches += 1;
+    L.op_epoch[d] = 0;
+  }
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return fail(ctx, B2D_ERR_CUDA, "kernel launch failed: %s", cudaGetErrorString(e));
+  return B2D_OK;
+}
+
+int b2d_bn_stats_exchange(b2d_ctx* ctx, int layer_id, const float* mean, const float* invstd, float count, float eps,
+                          float momentum, float* mean_out, float* invstd_out, int32_t* counts_out, float* running_mean,
+                          float* running_var, unsigned phases, void* stream) {
+  return bn_exchange(ctx, layer_id, true, mean, invstd, count, eps, momentum, mean_out, invstd_out, counts_out, running_mean,
+                     running_var, phases, stream);
+}
+
+int b2d_bn_grad_exchange(b2d_ctx* ctx, int layer_id, const float* sum_dy, const float* sum_dy_xmu, float* sum_dy_out,
+                         float* sum_dy_xmu_out, unsigned phases, void* stream) {
+  return bn_exchange(ctx, layer_id, false, sum_dy, sum_dy_xmu, 0.f, 0.f, 0.f, sum_dy_out, sum_dy_xmu_out, nullptr, nullptr,
+                     nullptr, phases, stream);
+}
+
 // ---- arena -------------------------------------------------------------------------------
 int b2d_arena_alloc(b2d_ctx* ctx, size_t bytes, void** dev_ptr, size_t* offset) {
   if (ctx == nullptr || dev_ptr == nullptr) return fail(ctx, B2D_ERR_INVALID, "NULL argument");
@@ -1712,6 +1821,7 @@ int b2d_arena_reset(b2d_ctx* ctx) {
   std::lock_guard<std::mutex> lk(ctx->mu);
   for (auto& kv : ctx->slots) for (cudaEvent_t e : kv.second.reuse_ev) if (e != nullptr) cudaEventDestroy(e);
   ctx->slots.clear();
+  ctx->bn_layers.clear();
   ctx->slot_free.clear();
   ctx->slot_top = kSignalBytes;
   ctx->user_bottom = ctx->arena_bytes;

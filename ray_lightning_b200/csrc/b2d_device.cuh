@@ -40,6 +40,9 @@ struct Signal {
   uint32_t staged[B2D_MAX_WORLD];
   uint32_t published[B2D_MAX_WORLD];
   uint32_t done_ctr[2];
+  // synchronised BatchNorm (b2d_syncbn.cuh): monotone exchange epochs, one word per source rank.  Separate from
+  // `staged`: the BN exchanges run on the caller's stream, concurrently with bucket exchanges on the internal ones.
+  uint32_t bn[B2D_MAX_WORLD];
 };
 static_assert(sizeof(Signal) <= 64 * 1024, "signal pad must fit its 64 KiB reservation");
 constexpr size_t kSignalBytes = 64 * 1024;

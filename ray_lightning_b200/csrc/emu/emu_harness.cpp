@@ -15,6 +15,7 @@
 #include "../b2d_kernels.cuh"
 #include "../b2d_staged.cuh"
 #include "../b2d_owner.cuh"
+#include "../b2d_syncbn.cuh"
 #include "../b2d_launch.cuh"
 
 thread_local EmuDim3 threadIdx, blockIdx, blockDim, gridDim;
@@ -438,6 +439,44 @@ int emu_owner_table(const long long* segs, int nseg, int world, int bf16, long l
   std::copy(t.start.begin(), t.start.end(), start);
   std::copy(t.owner_pack, t.owner_pack + world + 1, owner_pack);
   return static_cast<int>(t.flat_off.size());
+}
+
+// K15 + K16 (fwd = 1) or K15 + K17 (fwd = 0) of one BN exchange: rank r pushes (a[r], b[r], counts[r]) into the
+// region at region_off of every arena (a[r] / b[r] may be NULL: a zero row), then combines into out_a[r], out_b[r],
+// counts_out[r] and, when rm / rv are given, rank r's running statistics.  order as in emu_staged_allreduce (0 / 1).
+int emu_bn_exchange(void* h, int fwd, int channels, const float** a, const float** b, const float* counts, float eps, float momentum,
+                    float** out_a, float** out_b, int32_t** counts_out, float** rm, float** rv, size_t region_off, unsigned epoch,
+                    int grid, int order) {
+  Group* g = static_cast<Group*>(h);
+  const int world = g->world;
+  const size_t row = fwd ? bn_fwd_row(channels) : bn_bwd_row(channels);
+  if (region_off + static_cast<size_t>(world) * row * 4 > g->arena_bytes) return -4;
+  const Peers peers = make_peers(*g);
+  auto push = [&](int r) {
+    BnPushParams P{};
+    P.a = a[r]; P.b = b[r]; P.count = fwd ? counts[r] : 0.f; P.channels = channels; P.fwd = fwd;
+    P.region_off = region_off; P.rank = r; P.world = world; P.epoch = epoch; P.peers = peers;
+    return launch_one(1, kBnThreads, [P] { bn_push_kernel(P); });
+  };
+  auto combine = [&](int r) {
+    BnCombineParams P{};
+    P.region_off = region_off; P.channels = channels; P.eps = eps; P.momentum = momentum;
+    P.out_a = out_a[r]; P.out_b = out_b[r]; P.counts = fwd ? counts_out[r] : nullptr;
+    P.running_mean = rm ? rm[r] : nullptr; P.running_var = rv ? rv[r] : nullptr;
+    P.rank = r; P.world = world; P.epoch = epoch; P.timeout_ns = 120ull * 1000000000ull; P.diag = nullptr; P.peers = peers;
+    return fwd ? launch_one(grid, kBnThreads, [P] { bn_combine_kernel<true>(P); })
+               : launch_one(grid, kBnThreads, [P] { bn_combine_kernel<false>(P); });
+  };
+  if (order == 1) {
+    for (int r = 0; r < world; ++r) if (push(r) != 0) return -1;
+    for (int r = 0; r < world; ++r) if (combine(r) != 0) return -1;
+    return 0;
+  }
+  std::atomic<int> bad{0};
+  std::vector<std::thread> streams;
+  for (int r = 0; r < world; ++r) streams.emplace_back([&, r] { if (push(r) != 0 || combine(r) != 0) bad = 1; });
+  for (auto& t : streams) t.join();
+  return bad.load() ? -1 : 0;
 }
 
 float* emu_arena_ptr(void* h, int rank, size_t off) {

@@ -26,6 +26,9 @@ copy.  New knobs ride in as keyword arguments prefixed ``b200_`` and never reach
                               per step, one parameter group
     b200_enable=True
 
+``Trainer(sync_batchnorm=True)`` on the libb2d path converts every BatchNorm to ``syncbn.B200SyncBatchNorm``, whose
+statistics cross ranks through the arena; elsewhere it is torch's ``SyncBatchNorm``.
+
 There is no CPU implementation of that hook: with ``use_gpu=False`` the strategy is the
 reference's own CPU configuration (torch DDP over gloo), and with ``use_gpu=True`` a missing
 libb2d.so or GPU is an error, not a fallback.
@@ -169,6 +172,8 @@ class RayStrategy(DDPSpawnStrategy):
         self.b200_arena_buckets_active = False
         self._b200_rebuilt = False
         self._b200_steps = 0
+        if st is not None and self.root_device.type == "cuda" and self.world_size > 1:
+            self._setup_sync_batchnorm(st)
         if (st is None or not self._b200["arena_buckets"] or st.wire != "fp32" or self.root_device.type != "cuda"
                 or self.world_size < 2 or self._ddp_comm_wrapper is not None):
             return super().configure_ddp()
@@ -178,6 +183,30 @@ class RayStrategy(DDPSpawnStrategy):
         with st.allocate_in_arena():
             super().configure_ddp()
         self.b200_arena_buckets_active = st.verify_symmetric_buckets()
+
+    def configure_sync_batchnorm(self, model):
+        """``Trainer(sync_batchnorm=True)``: PL converts every BatchNorm before DDP wraps the model.  On the libb2d path
+        the layers become ``B200SyncBatchNorm`` (statistics exchanged by peer stores); otherwise — ``b200_enable=False``,
+        ``use_gpu=False`` or a comm hook of the user's — torch's ``SyncBatchNorm``, as in the reference."""
+        st = self.b200_state
+        if st is None or self.root_device.type != "cuda":
+            return super().configure_sync_batchnorm(model)
+        from .syncbn import convert_sync_batchnorm
+        return convert_sync_batchnorm(model, lambda: st.comm)
+
+    def _setup_sync_batchnorm(self, st):
+        """Collective, before the first forward: the communicator must exist with room for every layer's exchange
+        region, and the regions must be registered in the same order on every rank."""
+        from .syncbn import register_sync_batchnorm, sync_batchnorm_layers, syncbn_arena_bytes
+        layers = sync_batchnorm_layers(self.lightning_module)
+        if not layers:
+            return
+        if st.comm is None:
+            st.arena_extra_bytes += syncbn_arena_bytes([m.num_features for m in layers], self.world_size)
+        if st.total_grad_elems is None:
+            st.total_grad_elems = sum(p.numel() for p in self.model.parameters() if p.requires_grad)
+        st.ensure(self.root_device)
+        register_sync_batchnorm(self.lightning_module, st.comm)
 
     def training_step(self, *args):
         st = self.b200_state

@@ -43,14 +43,28 @@ class RayShardedStrategy(RayStrategy, DDPSpawnShardedStrategy):
         # consolidated checkpoints (4 B/element)
         wire = o["wire"] or ("bf16" if str(getattr(self, "precision", 32)) in ("16", "bf16") else "fp32")
         wire_w = 2 if wire == "bf16" else 4
-        nbytes = o["arena_bytes"] or int((8 + wire_w) * total + (128 << 20) + o["arena_extra_bytes"])
+        from .syncbn import register_sync_batchnorm, sync_batchnorm_layers, syncbn_arena_bytes
+        bn_layers = sync_batchnorm_layers(self.lightning_module) if self.world_size > 1 else []
+        bn_bytes = syncbn_arena_bytes([m.num_features for m in bn_layers], self.world_size)
+        nbytes = o["arena_bytes"] or int((8 + wire_w) * total + (128 << 20) + o["arena_extra_bytes"] + bn_bytes)
         self._comm = Communicator(self.global_rank, self.world_size, self.root_device.index, nbytes, mem=o["mem"],
                                   timing=o["timing"], max_ctas=o["max_ctas"], nvls=o["nvls"], timeout_ms=o["timeout_ms"],
                                   exch_ctas=o["exch_ctas"])
+        if bn_layers:
+            # no DDP wrapper broadcasts buffers here: synchronised statistics keep the running statistics equal
+            register_sync_batchnorm(self.lightning_module, self._comm)
         # the flat layout follows the optimizer's parameter groups: built in setup_optimizers, once they are known
         self.model = self.lightning_module
         self._sharded_wire = wire
         self._sharded_ready = True
+
+    def configure_sync_batchnorm(self, model):
+        """On the GPU the sharded path always has a libb2d communicator (created in configure_ddp): the layers become
+        ``B200SyncBatchNorm`` over it.  On the CPU reference path, torch's ``SyncBatchNorm``."""
+        if self.root_device.type != "cuda":
+            return DDPSpawnShardedStrategy.configure_sync_batchnorm(self, model)
+        from .syncbn import convert_sync_batchnorm
+        return convert_sync_batchnorm(model, lambda: getattr(self, "_comm", None))
 
     def _configure_cpu_reference(self):
         super().configure_ddp()
