@@ -313,6 +313,33 @@ int b2d_bn_stats_exchange(b2d_ctx* ctx, int layer_id, const float* mean, const f
 int b2d_bn_grad_exchange(b2d_ctx* ctx, int layer_id, const float* sum_dy, const float* sum_dy_xmu,
                          float* sum_dy_out, float* sum_dy_xmu_out, unsigned phases, void* stream);
 
+/* Replaces: the gradient multiply of OSS.clip_grad_norm / torch.nn.utils.clip_grad_norm_ (`grad.mul_(clip_coef)`, a
+ * separate pass over the gradients).  b2d_adam_push with every gradient of the own shard multiplied by *grad_scale
+ * (device fp32, non-NULL; one rounding) before the Adam update: the coefficient b2d_clip_norm wrote, read on the
+ * device, so the step needs no host synchronisation. */
+int b2d_adam_push_scaled(b2d_ctx* ctx, float* params, float* exp_avg, float* exp_avg_sq, const float* reduced, size_t n,
+                         const int64_t* shard_off, const b2d_adam_group* groups, int ngroups, unsigned flags,
+                         unsigned phases, void* wait_stream, void* comm_stream, const float* grad_scale);
+
+/* ---- gradient clipping (b2d_clip.cuh) ------------------------------------------------------ */
+
+/* Takes the clip exchange's region (two generations of W slots plus the per-block partials, a few KiB) from the arena
+ * and writes its arena offset to *offset (may be NULL).  Collective in the sense that every rank must call it at the
+ * same point, so that the offsets agree; calling it again is a no-op.  A context that never registers allocates and
+ * launches nothing for clipping.  Host only. */
+int b2d_clip_register(b2d_ctx* ctx, size_t* offset);
+
+/* Replaces: FairScale OSS.clip_grad_norm's local norm + NCCL all_reduce of its square (torch analogue:
+ * torch.nn.utils.clip_grad_norm_ with norm_type 2 over the whole gradient).  x: this rank's n fp32 elements (its
+ * reduced-gradient shard; n may be 0).  Every rank's sum of squares (fp64, an order fixed by n) reaches every rank;
+ * each combines them in rank order and writes, with identical bits on every rank,
+ *     norm_out[0] = fp32(sqrt(sum))    coef_out[0] = min(max_norm * (1 / (norm + 1e-6)), 1)   (NaN kept)
+ * (device fp32).  max_norm must be finite and >= 0.  Asynchronous on the library's internal stream behind the reduce
+ * buckets, after `wait_stream`; `comm_stream` waits for the result.  phases: bit 0 partial + push, bit 1 wait +
+ * coefficient (3 = both); hosts that drive several ranks from one thread issue bit 0 for every rank, then bit 1. */
+int b2d_clip_norm(b2d_ctx* ctx, const float* x, size_t n, float max_norm, float* norm_out, float* coef_out,
+                  unsigned phases, void* wait_stream, void* comm_stream);
+
 /* ---- symmetric arena ------------------------------------------------------------------- */
 
 /* Bump-allocate `bytes` (256-byte aligned) of caller-visible symmetric memory.  Every rank

@@ -35,6 +35,7 @@ EXPORTED_SYMBOLS = [
     "b2d_peer_bw", "b2d_pool_bind", "b2d_pool_alloc", "b2d_pool_free", "b2d_ctx_set_inplace",
     "b2d_bucket_register", "b2d_reduce_to_owner", "b2d_adam_push", "b2d_ctx_set_auto_profile",
     "b2d_optim_register", "b2d_bucket_optim", "b2d_bn_register", "b2d_bn_stats_exchange", "b2d_bn_grad_exchange",
+    "b2d_adam_push_scaled", "b2d_clip_register", "b2d_clip_norm",
 ]
 PROFILE_OVERLAP, PROFILE_LATENCY = 0, 1
 RTO_ZERO_GRADS, RTO_ACCUMULATE, RTO_NVLS = 1, 2, 4
@@ -122,6 +123,10 @@ def _declare(lib):
                              c.POINTER(AdamParams), vp, vp],
         "b2d_reduce_scatter": [vp, c.c_int, vp, vp, sz, c.POINTER(c.c_int64), c.c_int, c.c_float, vp, vp],
         "b2d_allgather": [vp, vp, sz, c.POINTER(c.c_int64), vp, vp],
+        "b2d_adam_push_scaled": [vp, vp, vp, vp, vp, sz, c.POINTER(c.c_int64), c.POINTER(AdamGroup), c.c_int, c.c_uint,
+                                 c.c_uint, vp, vp, vp],
+        "b2d_clip_register": [vp, c.POINTER(sz)],
+        "b2d_clip_norm": [vp, vp, sz, c.c_float, vp, vp, c.c_uint, vp, vp],
         "b2d_bn_register": [vp, c.c_int, c.c_int, c.POINTER(sz)],
         "b2d_bn_stats_exchange": [vp, c.c_int, vp, vp, c.c_float, c.c_float, c.c_float, vp, vp, vp, vp, vp, c.c_uint, vp],
         "b2d_bn_grad_exchange": [vp, c.c_int, vp, vp, vp, vp, c.c_uint, vp],
@@ -329,14 +334,30 @@ class Context:
                                                   ctypes.c_void_p(reduced_ptr), off, float(scale), int(flags), int(phases),
                                                   _stream_ptr(wait_stream), _stream_ptr(comm_stream)))
 
-    def adam_push(self, params_ptr, m_ptr, v_ptr, reduced_ptr, n, shard_off, groups, flags, wait_stream, comm_stream, phases=6):
-        """groups: list of (lo, hi, AdamParams) relative to the own shard; empty: push only."""
+    def adam_push(self, params_ptr, m_ptr, v_ptr, reduced_ptr, n, shard_off, groups, flags, wait_stream, comm_stream, phases=6,
+                  grad_scale_ptr=None):
+        """groups: list of (lo, hi, AdamParams) relative to the own shard; empty: push only.  grad_scale_ptr: device fp32
+        factor for the gradients (b2d_adam_push_scaled)."""
         off = (ctypes.c_int64 * len(shard_off))(*[int(x) for x in shard_off])
         arr = (AdamGroup * max(len(groups), 1))(*[AdamGroup(int(lo), int(hi), a, 0) for lo, hi, a in groups])
-        self._check(self._lib.b2d_adam_push(self._ctx, ctypes.c_void_p(params_ptr), ctypes.c_void_p(m_ptr or 0),
-                                            ctypes.c_void_p(v_ptr or 0), ctypes.c_void_p(reduced_ptr or 0), int(n), off, arr,
-                                            len(groups), int(flags), int(phases), _stream_ptr(wait_stream),
-                                            _stream_ptr(comm_stream)))
+        args = (self._ctx, ctypes.c_void_p(params_ptr), ctypes.c_void_p(m_ptr or 0), ctypes.c_void_p(v_ptr or 0),
+                ctypes.c_void_p(reduced_ptr or 0), int(n), off, arr, len(groups), int(flags), int(phases),
+                _stream_ptr(wait_stream), _stream_ptr(comm_stream))
+        if grad_scale_ptr is None:
+            self._check(self._lib.b2d_adam_push(*args))
+        else:
+            self._check(self._lib.b2d_adam_push_scaled(*args, ctypes.c_void_p(grad_scale_ptr)))
+
+    def clip_register(self):
+        """Returns the arena offset of the clip exchange's region."""
+        off = ctypes.c_size_t()
+        self._check(self._lib.b2d_clip_register(self._ctx, ctypes.byref(off)))
+        return off.value
+
+    def clip_norm(self, x_ptr, n, max_norm, norm_ptr, coef_ptr, phases, wait_stream, comm_stream):
+        vp = ctypes.c_void_p
+        self._check(self._lib.b2d_clip_norm(self._ctx, vp(x_ptr), int(n), float(max_norm), vp(norm_ptr), vp(coef_ptr),
+                                            int(phases), _stream_ptr(wait_stream), _stream_ptr(comm_stream)))
 
     def optim_register(self, bucket_id, param_ptrs, state1_ptrs, state2_ptrs, bucket_offs, numels):
         n = len(param_ptrs)

@@ -183,6 +183,15 @@ class ModelCheckpoint(Callback):
         self.best_model_path, self.best_model_score = path, score
 
 
+def _clip_algorithm(algorithm):
+    """PL's GradClipAlgorithmType: "norm" (the default) or "value"."""
+    if algorithm is None:
+        return "norm"
+    if algorithm not in ("norm", "value"):
+        raise ValueError("gradient_clip_algorithm %r is invalid: allowed values are 'norm' and 'value'" % (algorithm,))
+    return algorithm
+
+
 # ---- module / datamodule ---------------------------------------------------------------------------
 class LightningModule(nn.Module):
     def __init__(self):
@@ -195,6 +204,16 @@ class LightningModule(nn.Module):
     def training_step(self, batch, batch_idx): raise NotImplementedError
     def configure_optimizers(self): raise NotImplementedError
     def on_save_checkpoint(self, checkpoint): pass
+
+    def configure_gradient_clipping(self, optimizer, optimizer_idx, gradient_clip_val=None, gradient_clip_algorithm=None):
+        """PL 1.6 hook, called after backward and before each optimizer step when the Trainer clips."""
+        self.clip_gradients(optimizer, gradient_clip_val=gradient_clip_val, gradient_clip_algorithm=gradient_clip_algorithm)
+
+    def clip_gradients(self, optimizer, gradient_clip_val=None, gradient_clip_algorithm=None):
+        if gradient_clip_val is None or gradient_clip_val <= 0:
+            return
+        algorithm = _clip_algorithm(gradient_clip_algorithm)
+        self.trainer.strategy.clip_gradients(optimizer, float(gradient_clip_val), algorithm)
     def on_load_checkpoint(self, checkpoint): pass
     def prepare_data(self): pass
     def setup(self, stage=None): pass
@@ -348,6 +367,14 @@ class Strategy:
 
     def optimizer_step(self, optimizer):
         optimizer.step()
+
+    def clip_gradients(self, optimizer, clip_val, algorithm="norm"):
+        """torch's clip_grad_norm_ (norm_type 2) or clip_grad_value_ over the parameters of the optimizer's groups."""
+        params = [p for g in optimizer.param_groups for p in g["params"]]
+        if algorithm == "value":
+            torch.nn.utils.clip_grad_value_(params, clip_val)
+        else:
+            torch.nn.utils.clip_grad_norm_(params, clip_val)
 
     def barrier(self, name=None):
         pass
@@ -526,7 +553,8 @@ class Trainer:
                  limit_train_batches=1.0, limit_val_batches=1.0, limit_test_batches=1.0, enable_progress_bar=False,
                  checkpoint_callback=None, enable_checkpointing=True, precision=32, num_sanity_val_steps=0,
                  resume_from_checkpoint=None, reload_dataloaders_every_n_epochs=0, gpus=None, logger=None,
-                 progress_bar_refresh_rate=None, log_every_n_steps=50, sync_batchnorm=False, **_ignored):
+                 progress_bar_refresh_rate=None, log_every_n_steps=50, sync_batchnorm=False, gradient_clip_val=None,
+                 gradient_clip_algorithm=None, **_ignored):
         self.default_root_dir = str(default_root_dir) if default_root_dir is not None else os.getcwd()
         self.callbacks = list(callbacks or [])
         if checkpoint_callback is not None:
@@ -536,6 +564,8 @@ class Trainer:
         self.strategy = strategy if strategy is not None else Strategy()
         self.strategy.precision = precision
         self.strategy.sync_batchnorm = bool(sync_batchnorm)
+        self.gradient_clip_algorithm = _clip_algorithm(gradient_clip_algorithm)
+        self.gradient_clip_val = gradient_clip_val
         self.max_epochs, self.max_steps = max_epochs, max_steps
         self.limit_train_batches, self.limit_val_batches, self.limit_test_batches = \
             limit_train_batches, limit_val_batches, limit_test_batches
@@ -723,6 +753,10 @@ class Trainer:
                 out = self.strategy.training_step(batch, batch_idx)
                 loss = out["loss"] if isinstance(out, dict) else out
                 self.strategy.backward(loss)
+                if self.gradient_clip_val is not None and self.gradient_clip_val > 0:
+                    for i, opt in enumerate(self.strategy.optimizers):
+                        model.configure_gradient_clipping(opt, i, gradient_clip_val=self.gradient_clip_val,
+                                                          gradient_clip_algorithm=self.gradient_clip_algorithm)
                 for opt in self.strategy.optimizers:
                     self.strategy.optimizer_step(opt)
                 self.global_step += 1

@@ -182,18 +182,42 @@ class _Base:
         self.ctx.reduce_to_owner(bucket_id, grads.data_ptr(), reduced.data_ptr(), shard_off, scale, flags, ws, cs, phases)
 
     def adam_push_(self, params, exp_avg, exp_avg_sq, reduced, shard_off, groups, nvls=False, wait_stream=None,
-                   comm_stream=None, phases=6):
+                   comm_stream=None, phases=6, grad_scale=None):
         """Adam / AdamW on the own shard per parameter group, new parameters pushed into every rank's flat buffer
-        (``groups`` = [(lo, hi, dict(lr, beta1, beta2, eps, weight_decay, step, adamw))], empty: push only)."""
+        (``groups`` = [(lo, hi, dict(lr, beta1, beta2, eps, weight_decay, step, adamw))], empty: push only).
+        ``grad_scale``: a one-element fp32 device tensor every gradient is multiplied by first (the clip coefficient
+        of ``clip_norm_``; b2d_adam_push_scaled)."""
         _check_tensor(params, self.device_index)
+        if grad_scale is not None:
+            _check_tensor(grad_scale, self.device_index)
         ws = torch.cuda.current_stream(params.device) if wait_stream is None else wait_stream
         cs = ws if comm_stream is None else comm_stream
         gs = [(lo, hi, AdamParams(lr=a["lr"], beta1=a["beta1"], beta2=a["beta2"], eps=a["eps"],
                                   weight_decay=a["weight_decay"], step=int(a["step"]), adamw=int(a["adamw"]), zero_grads=0))
               for lo, hi, a in groups]
         ptr = lambda t: 0 if t is None else t.data_ptr()
-        self.ctx.adam_push(params.data_ptr(), ptr(exp_avg), ptr(exp_avg_sq), ptr(reduced), params.numel(), shard_off, gs,
-                           _b2d.RTO_NVLS if nvls else 0, ws, cs, phases)
+        if grad_scale is None:
+            self.ctx.adam_push(params.data_ptr(), ptr(exp_avg), ptr(exp_avg_sq), ptr(reduced), params.numel(), shard_off, gs,
+                               _b2d.RTO_NVLS if nvls else 0, ws, cs, phases)
+        else:
+            self.ctx.adam_push(params.data_ptr(), ptr(exp_avg), ptr(exp_avg_sq), ptr(reduced), params.numel(), shard_off, gs,
+                               _b2d.RTO_NVLS if nvls else 0, ws, cs, phases, grad_scale_ptr=grad_scale.data_ptr())
+
+    # ---- gradient clipping (b2d_clip.cuh) --------------------------------------------------------------------
+    def clip_register(self):
+        """Give the clip exchange its region in the arena (once; later calls return the same offset)."""
+        return self.ctx.clip_register()
+
+    def clip_norm_(self, x, max_norm, norm_out, coef_out, wait_stream=None, comm_stream=None, phases=3):
+        """Global 2-norm of every rank's ``x`` (its reduced-gradient shard; may be empty) into ``norm_out`` and torch's
+        clip coefficient ``min(max_norm / (norm + 1e-6), 1)`` into ``coef_out`` (one-element fp32 device tensors), with
+        identical bits on every rank.  Asynchronous after ``wait_stream``; ``comm_stream`` waits for the result."""
+        _check_tensor(x, self.device_index)
+        _check_tensor(norm_out, self.device_index)
+        _check_tensor(coef_out, self.device_index)
+        ws = torch.cuda.current_stream(x.device) if wait_stream is None else wait_stream
+        cs = ws if comm_stream is None else comm_stream
+        self.ctx.clip_norm(x.data_ptr(), x.numel(), float(max_norm), norm_out.data_ptr(), coef_out.data_ptr(), phases, ws, cs)
 
     def allgather_(self, buf, shard_off, wait_stream=None, comm_stream=None):
         _check_tensor(buf, self.device_index)
@@ -391,6 +415,18 @@ class Communicator(_Base):
                                    "rank must register the same layers in the same order")
         return offs
 
+    def clip_register(self):
+        """Collective: register the clip region and check over the control plane that it sits at the same arena offset
+        on every rank."""
+        off = super().clip_register()
+        if self.world > 1 and dist.is_initialized():
+            allv = [None] * self.world
+            dist.all_gather_object(allv, off, group=self.group)
+            if any(v != off for v in allv):
+                raise RuntimeError("the clip region landed at different arena offsets on different ranks (%s): every rank "
+                                   "must clip at the same step" % allv)
+        return off
+
     def close(self):
         if self.ctx is not None:
             if self.world > 1 and dist.is_initialized():
@@ -480,13 +516,29 @@ class LoopbackGroup:
                 rk.reduce_to_owner(bucket_id, grads[r], reduced[r], shard_off, phases=ph,
                                    wait_stream=torch.cuda.current_stream(grads[r].device), comm_stream=rk.stream, **kw)
 
-    def adam_push_(self, params, exp_avg, exp_avg_sq, reduced, shard_off, groups, **kw):
-        """groups[r]: rank r's parameter-group list.  Phase-major: step + push everywhere, then wait everywhere."""
+    def adam_push_(self, params, exp_avg, exp_avg_sq, reduced, shard_off, groups, grad_scale=None, **kw):
+        """groups[r]: rank r's parameter-group list; grad_scale[r] (optional): rank r's gradient factor.  Phase-major:
+        step + push everywhere, then wait everywhere."""
         for ph in (2, 4):
             for r, rk in enumerate(self.ranks):
                 rk.adam_push_(params[r], None if exp_avg is None else exp_avg[r], None if exp_avg_sq is None else exp_avg_sq[r],
                               None if reduced is None else reduced[r], shard_off, groups[r], phases=ph,
-                              wait_stream=torch.cuda.current_stream(params[r].device), comm_stream=rk.stream, **kw)
+                              wait_stream=torch.cuda.current_stream(params[r].device), comm_stream=rk.stream,
+                              grad_scale=None if grad_scale is None else grad_scale[r], **kw)
+
+    def clip_register(self):
+        offs = [rk.clip_register() for rk in self.ranks]
+        if len(set(offs)) != 1:
+            raise RuntimeError("clip region at different arena offsets: %s" % offs)
+        return offs[0]
+
+    def clip_norm_(self, xs, max_norm, norm_outs, coef_outs):
+        """Rank r's shard is xs[r].  Phase-major on the ranks' own streams (after the current stream): every partial,
+        then every coefficient."""
+        for ph in (1, 2):
+            for r, rk in enumerate(self.ranks):
+                rk.clip_norm_(xs[r], max_norm, norm_outs[r], coef_outs[r], phases=ph,
+                              wait_stream=torch.cuda.current_stream(xs[r].device), comm_stream=rk.stream)
 
     def reduce_scatter(self, grads, outs, shard_off, **kw):
         for r, rk in enumerate(self.ranks):

@@ -22,6 +22,7 @@
 #include "b2d_staged.cuh"
 #include "b2d_owner.cuh"
 #include "b2d_syncbn.cuh"
+#include "b2d_clip.cuh"
 #include "b2d_launch.cuh"
 
 using namespace b2d;
@@ -240,6 +241,13 @@ struct b2d_ctx {
   };
   std::map<int, BnLayer> bn_layers;
   uint32_t bn_epoch = 0;   // the BN exchanges' own epoch (Signal::bn), independent of the bucket exchanges' `epoch`
+
+  // gradient clipping (b2d_clip.cuh): one arena region, [gen 0: W slots | gen 1: W slots | kClipGMax block sums],
+  // taken by b2d_clip_register.  clip_op_epoch != 0 while a pushed partial waits for its combine phase.
+  bool clip_registered = false;
+  size_t clip_off = 0;
+  unsigned clip_calls = 0, clip_gen = 0;
+  uint32_t clip_epoch = 0, clip_op_epoch = 0;   // Signal::clip's own epoch, independent of `epoch` and `bn_epoch`
 
   unsigned long long* trace_dev = nullptr;   // debug: per-block phase stamps of the LAST allreduce launch
   int trace_grid = 0;
@@ -670,6 +678,7 @@ const auto preload_owner = [](auto w) {
   preload_one(seg_reduce_kernel<W, true, false>); preload_one(seg_reduce_kernel<W, true, true>);
   preload_one(seg_reduce_kernel<W, false, false>); preload_one(seg_reduce_kernel<W, false, true>);
   preload_one(adam_push_kernel<W, false>); preload_one(adam_push_kernel<W, true>);
+  preload_one(adam_push_scaled_kernel<W, false>); preload_one(adam_push_scaled_kernel<W, true>);
 };
 const auto tma_attr = [](auto w) {
   if (cudaFuncSetAttribute(k2t_two_shot_tma_kernel<decltype(w)::value, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kTmaSmemBytes) != cudaSuccess)
@@ -686,6 +695,7 @@ void preload_kernels() {
   for (int world : worlds) dispatch_world(world, preload_owner);
   preload_one(bucket_optim_kernel);
   preload_one(bn_push_kernel); preload_one(bn_combine_kernel<true>); preload_one(bn_combine_kernel<false>);
+  preload_one(sqnorm_partial_kernel); preload_one(clip_coef_kernel);
   preload_one(k0_cast_scale_kernel<true>);
   preload_one(k0_cast_scale_kernel<false>);
   preload_one(barrier_kernel);
@@ -1569,9 +1579,10 @@ int b2d_reduce_to_owner(b2d_ctx* ctx, int bucket_id, float* grads, float* reduce
   return B2D_OK;
 }
 
-int b2d_adam_push(b2d_ctx* ctx, float* params, float* exp_avg, float* exp_avg_sq, const float* reduced, size_t n,
-                  const int64_t* shard_off, const b2d_adam_group* groups, int ngroups, unsigned flags, unsigned phases,
-                  void* wait_stream, void* comm_stream) {
+// b2d_adam_push (grad_scale == NULL: K13) and b2d_adam_push_scaled (K13 with the gradients scaled on the device)
+static int adam_push(b2d_ctx* ctx, float* params, float* exp_avg, float* exp_avg_sq, const float* reduced, size_t n,
+                     const int64_t* shard_off, const b2d_adam_group* groups, int ngroups, unsigned flags, unsigned phases,
+                     void* wait_stream, void* comm_stream, const float* grad_scale) {
   int rc = check_ready(ctx);
   if (rc != B2D_OK) return rc;
   std::lock_guard<std::mutex> lk(ctx->mu);
@@ -1610,6 +1621,7 @@ int b2d_adam_push(b2d_ctx* ctx, float* params, float* exp_avg, float* exp_avg_sq
       P.group[k] = adam_consts(groups[k].adam);
     }
     P.rank = ctx->rank; P.world = ctx->world; P.epoch = ctx->push_epoch; P.peers = ctx->peers;
+    P.grad_scale = grad_scale;
     rc = stream_wait(ctx, ctx->s_xfer, static_cast<cudaStream_t>(wait_stream));
     if (rc != B2D_OK) return rc;
     // the step is not overlapped with anything and moves 28 B of local HBM traffic per owned element: one full wave
@@ -1620,7 +1632,11 @@ int b2d_adam_push(b2d_ctx* ctx, float* params, float* exp_avg, float* exp_avg_sq
     if (timing) B2D_CUDA(ctx, cudaEventRecord(tp.first, ctx->s_xfer));
     dispatch_world(ctx->world, [&](auto w) {
       constexpr int W = decltype(w)::value;
-      if (nvls) adam_push_kernel<W, true><<<grid, kExThreads, 0, ctx->s_xfer>>>(P); else adam_push_kernel<W, false><<<grid, kExThreads, 0, ctx->s_xfer>>>(P);
+      if (grad_scale != nullptr) {
+        if (nvls) adam_push_scaled_kernel<W, true><<<grid, kExThreads, 0, ctx->s_xfer>>>(P); else adam_push_scaled_kernel<W, false><<<grid, kExThreads, 0, ctx->s_xfer>>>(P);
+      } else {
+        if (nvls) adam_push_kernel<W, true><<<grid, kExThreads, 0, ctx->s_xfer>>>(P); else adam_push_kernel<W, false><<<grid, kExThreads, 0, ctx->s_xfer>>>(P);
+      }
     });
     ctx->launches += 1;
     if (timing) { B2D_CUDA(ctx, cudaEventRecord(tp.second, ctx->s_xfer)); ctx->ev_pending.push_back(tp); }
@@ -1642,6 +1658,89 @@ int b2d_adam_push(b2d_ctx* ctx, float* params, float* exp_avg, float* exp_avg_sq
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return fail(ctx, B2D_ERR_CUDA, "kernel launch failed: %s", cudaGetErrorString(e));
   ctx->last_algo = 13; ctx->last_block = kExThreads;
+  return B2D_OK;
+}
+
+int b2d_adam_push(b2d_ctx* ctx, float* params, float* exp_avg, float* exp_avg_sq, const float* reduced, size_t n,
+                  const int64_t* shard_off, const b2d_adam_group* groups, int ngroups, unsigned flags, unsigned phases,
+                  void* wait_stream, void* comm_stream) {
+  return adam_push(ctx, params, exp_avg, exp_avg_sq, reduced, n, shard_off, groups, ngroups, flags, phases, wait_stream,
+                   comm_stream, nullptr);
+}
+
+int b2d_adam_push_scaled(b2d_ctx* ctx, float* params, float* exp_avg, float* exp_avg_sq, const float* reduced, size_t n,
+                         const int64_t* shard_off, const b2d_adam_group* groups, int ngroups, unsigned flags, unsigned phases,
+                         void* wait_stream, void* comm_stream, const float* grad_scale) {
+  if (grad_scale == nullptr) return fail(ctx, B2D_ERR_INVALID, "grad_scale is NULL");
+  return adam_push(ctx, params, exp_avg, exp_avg_sq, reduced, n, shard_off, groups, ngroups, flags, phases, wait_stream,
+                   comm_stream, grad_scale);
+}
+
+// ---- gradient clipping (b2d_clip.cuh) ------------------------------------------------------------------------------
+static_assert(kClipGMax <= static_cast<unsigned>(kClipThreads), "K18's final tree combines at most kClipThreads block sums");
+
+int b2d_clip_register(b2d_ctx* ctx, size_t* offset) {
+  if (ctx == nullptr) return fail(nullptr, B2D_ERR_INVALID, "ctx is NULL");
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  if (!ctx->clip_registered) {
+    const size_t bytes = round_up(2 * static_cast<size_t>(ctx->world) * kClipSlotBytes + kClipGMax * sizeof(double), kAlign);
+    size_t off = 0;
+    if (!slot_region_alloc(ctx, bytes, &off))
+      return fail(ctx, B2D_ERR_NOMEM, "symmetric arena exhausted: the clip region needs %zu bytes, %zu free of %zu", bytes,
+                  ctx->user_bottom - ctx->slot_top, ctx->arena_bytes);
+    ctx->clip_off = off;
+    ctx->clip_registered = true;
+  }
+  if (offset != nullptr) *offset = ctx->clip_off;
+  return B2D_OK;
+}
+
+int b2d_clip_norm(b2d_ctx* ctx, const float* x, size_t n, float max_norm, float* norm_out, float* coef_out, unsigned phases,
+                  void* wait_stream, void* comm_stream) {
+  int rc = check_ready(ctx);
+  if (rc != B2D_OK) return rc;
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  if (!ctx->clip_registered) return fail(ctx, B2D_ERR_STATE, "b2d_clip_norm before b2d_clip_register");
+  if ((phases & 3u) == 0 || phases > 3u) return fail(ctx, B2D_ERR_INVALID, "bad phase mask %u (bit 0 partial, bit 1 coefficient)", phases);
+  if (!(max_norm >= 0.f) || !isfinite(max_norm)) return fail(ctx, B2D_ERR_INVALID, "max_norm must be finite and >= 0 (got %g)", static_cast<double>(max_norm));
+  if ((phases & 1u) && n > 0 && x == nullptr) return fail(ctx, B2D_ERR_INVALID, "x is NULL");
+  if ((phases & 2u) && (norm_out == nullptr || coef_out == nullptr)) return fail(ctx, B2D_ERR_INVALID, "NULL output");
+  if ((phases & 1u) && ctx->clip_op_epoch != 0) return fail(ctx, B2D_ERR_STATE, "clip partial issued again before the previous one was combined");
+  if (!(phases & 1u) && ctx->clip_op_epoch == 0) return fail(ctx, B2D_ERR_STATE, "clip coefficient issued before the partial");
+  DeviceGuard guard(ctx->device);
+  if (!guard.ok) return fail(ctx, B2D_ERR_CUDA, "cudaSetDevice(%d) failed", ctx->device);
+  rc = ensure_streams(ctx);
+  if (rc != B2D_OK) return rc;
+  // on s_xfer, behind the reduce buckets (K12) that wrote the shard
+  const size_t gen_bytes = static_cast<size_t>(ctx->world) * kClipSlotBytes;
+  if (phases & 1u) {
+    rc = stream_wait(ctx, ctx->s_xfer, static_cast<cudaStream_t>(wait_stream));
+    if (rc != B2D_OK) return rc;
+    ctx->clip_gen = ctx->clip_calls++ & 1u;
+    ctx->clip_op_epoch = ++ctx->clip_epoch;
+    ClipPartialParams P{};
+    P.x = x; P.n = n; P.vec = (reinterpret_cast<uintptr_t>(x) % 16) == 0;
+    P.block_sums = reinterpret_cast<double*>(ctx->arena + ctx->clip_off + 2 * gen_bytes);
+    P.region_off = ctx->clip_off + ctx->clip_gen * gen_bytes;
+    P.rank = ctx->rank; P.world = ctx->world; P.epoch = ctx->clip_op_epoch; P.peers = ctx->peers;
+    sqnorm_partial_kernel<<<clip_grid(n, kClipGMax), kClipThreads, 0, ctx->s_xfer>>>(P);
+    ctx->launches += 1;
+  }
+  if (phases & 2u) {
+    ClipCoefParams P{};
+    P.region_off = ctx->clip_off + ctx->clip_gen * gen_bytes;
+    P.max_norm = max_norm; P.norm_out = norm_out; P.coef_out = coef_out;
+    set_peer_wait(ctx, &P);
+    P.epoch = ctx->clip_op_epoch;
+    clip_coef_kernel<<<1, 32, 0, ctx->s_xfer>>>(P);
+    ctx->launches += 1;
+    cudaEvent_t ex = next_event(ctx);
+    B2D_CUDA(ctx, cudaEventRecord(ex, ctx->s_xfer));
+    B2D_CUDA(ctx, cudaStreamWaitEvent(static_cast<cudaStream_t>(comm_stream), ex, 0));
+    ctx->clip_op_epoch = 0;
+  }
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return fail(ctx, B2D_ERR_CUDA, "kernel launch failed: %s", cudaGetErrorString(e));
   return B2D_OK;
 }
 
@@ -1822,6 +1921,8 @@ int b2d_arena_reset(b2d_ctx* ctx) {
   for (auto& kv : ctx->slots) for (cudaEvent_t e : kv.second.reuse_ev) if (e != nullptr) cudaEventDestroy(e);
   ctx->slots.clear();
   ctx->bn_layers.clear();
+  ctx->clip_registered = false;
+  ctx->clip_op_epoch = 0;
   ctx->slot_free.clear();
   ctx->slot_top = kSignalBytes;
   ctx->user_bottom = ctx->arena_bytes;

@@ -43,6 +43,10 @@ struct Signal {
   // synchronised BatchNorm (b2d_syncbn.cuh): monotone exchange epochs, one word per source rank.  Separate from
   // `staged`: the BN exchanges run on the caller's stream, concurrently with bucket exchanges on the internal ones.
   uint32_t bn[B2D_MAX_WORLD];
+  // gradient clipping (b2d_clip.cuh): monotone clip-exchange epochs, one word per source rank, with their own host
+  // epoch counter; clip_ctr is K18's local "blocks finished" ticket (not done_ctr: K11 / K13 share those)
+  uint32_t clip[B2D_MAX_WORLD];
+  uint32_t clip_ctr;
 };
 static_assert(sizeof(Signal) <= 64 * 1024, "signal pad must fit its 64 KiB reservation");
 constexpr size_t kSignalBytes = 64 * 1024;

@@ -27,6 +27,10 @@ void dispatch_world(int world, F&& f) {
   }
 }
 
+// Most blocks the global-norm kernel K18 (b2d_clip.cuh) runs: its summation order depends on this value and on the
+// element count only, never on the device.  At most kClipThreads, the width of the final tree.
+constexpr unsigned kClipGMax = 256;
+
 // Python-float (double) arithmetic of torch/optim/adam.py:503-541, cast once.
 inline AdamConsts adam_consts(const b2d_adam& adam) {
   AdamConsts a{};

@@ -169,16 +169,20 @@ struct PushParams {
   int rank, world;
   uint32_t epoch;
   Peers peers;
+  const float* grad_scale;   // adam_push_scaled_kernel: device fp32 factor applied to every gradient (clip coefficient)
 };
 
-template <int W, bool NVLS>
-__global__ void __launch_bounds__(kExThreads, 2) adam_push_kernel(const __grid_constant__ PushParams P) {
+// SCALED: g = g * (*grad_scale) before the update, one rounding — torch's `grad.mul_(clip_coef)` followed by the step
+template <int W, bool NVLS, bool SCALED>
+__device__ __forceinline__ void adam_push_body(const PushParams& P) {
   constexpr int WW = W > 0 ? W : B2D_MAX_WORLD;
   const int world = W > 0 ? W : P.world;
   const size_t nv = static_cast<size_t>(P.hi - P.lo) / 4;   // 16-byte vectors of the own shard
   const size_t gt = static_cast<size_t>(gridDim.x) * blockDim.x;
   const size_t g = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
   constexpr int U = 2;
+  float gscale = 1.f;
+  if constexpr (SCALED) gscale = *P.grad_scale;
   for (size_t j = g; j < nv; j += gt * U) {
     uint4 pr[U], gr[U], mr[U], vr[U];
 #pragma unroll
@@ -207,6 +211,10 @@ __global__ void __launch_bounds__(kExThreads, 2) adam_push_kernel(const __grid_c
             float gg[4] = {__uint_as_float(gr[u].x), __uint_as_float(gr[u].y), __uint_as_float(gr[u].z), __uint_as_float(gr[u].w)};
             float mm[4] = {__uint_as_float(mr[u].x), __uint_as_float(mr[u].y), __uint_as_float(mr[u].z), __uint_as_float(mr[u].w)};
             float vv[4] = {__uint_as_float(vr[u].x), __uint_as_float(vr[u].y), __uint_as_float(vr[u].z), __uint_as_float(vr[u].w)};
+            if constexpr (SCALED) {
+#pragma unroll
+              for (int k = 0; k < 4; ++k) gg[k] = __fmul_rn(gg[k], gscale);
+            }
 #pragma unroll
             for (int k = 0; k < 4; ++k) adam_update(gg[k], pp[k], mm[k], vv[k], P.group[gi]);
             out = make_uint4(__float_as_uint(pp[0]), __float_as_uint(pp[1]), __float_as_uint(pp[2]), __float_as_uint(pp[3]));
@@ -226,6 +234,17 @@ __global__ void __launch_bounds__(kExThreads, 2) adam_push_kernel(const __grid_c
     }
   }
   arrive_when_grid_done(P.peers, P.rank, P.world, 1, P.epoch);
+}
+
+template <int W, bool NVLS>
+__global__ void __launch_bounds__(kExThreads, 2) adam_push_kernel(const __grid_constant__ PushParams P) {
+  adam_push_body<W, NVLS, false>(P);
+}
+
+// K13 with the clip coefficient of K19 (b2d_clip.cuh) applied to the gradients
+template <int W, bool NVLS>
+__global__ void __launch_bounds__(kExThreads, 2) adam_push_scaled_kernel(const __grid_constant__ PushParams P) {
+  adam_push_body<W, NVLS, true>(P);
 }
 
 // ---- K14: optimizer step of one DDP bucket, right behind its allreduce (SURVEY §8 f-2) --------------------------

@@ -14,7 +14,7 @@ PKG = os.path.dirname(HERE)
 LIB_DIR = os.path.join(PKG, "lib")
 LIB_PATH = os.path.join(LIB_DIR, "libb2d.so")
 SOURCES = ["b2d.cu"]
-HEADERS = ["b2d_device.cuh", "b2d_kernels.cuh", "b2d_tma.cuh", "b2d_staged.cuh", "b2d_owner.cuh", "b2d_syncbn.cuh", "b2d_launch.cuh", os.path.join("..", "..", "include", "b2d.h")]
+HEADERS = ["b2d_device.cuh", "b2d_kernels.cuh", "b2d_tma.cuh", "b2d_staged.cuh", "b2d_owner.cuh", "b2d_syncbn.cuh", "b2d_clip.cuh", "b2d_launch.cuh", os.path.join("..", "..", "include", "b2d.h")]
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",

@@ -45,6 +45,7 @@ struct Block {
   explicit Block(int nthreads) : n(nthreads), bar0(nthreads) {}
   int n;
   int scratch = 0;   // stands in for a __shared__ int (b2d_staged.cuh: "was this the last block?")
+  double dscratch[256] = {};   // stands in for a __shared__ double[256] (b2d_clip.cuh: the block's summation tree)
   std::barrier<> bar0;
   std::mutex mu;
   std::map<int, std::unique_ptr<std::barrier<>>> named;  // id -> barrier(count)
@@ -101,6 +102,11 @@ inline float __fadd_rn(float a, float b) { volatile float r = a + b; return r; }
 inline float __fmul_rn(float a, float b) { volatile float r = a * b; return r; }   // no contraction, one rounding
 inline float __fdiv_rn(float a, float b) { volatile float r = a / b; return r; }
 inline float __fsqrt_rn(float a) { volatile float r = std::sqrt(a); return r; }
+inline float __frcp_rn(float a) { volatile float r = 1.f / a; return r; }
+inline double __dadd_rn(double a, double b) { volatile double r = a + b; return r; }
+inline double __dmul_rn(double a, double b) { volatile double r = a * b; return r; }
+inline double __dsqrt_rn(double a) { volatile double r = std::sqrt(a); return r; }
+inline float __double2float_rn(double a) { volatile float r = static_cast<float>(a); return r; }
 
 // fp32 -> bf16 bits, round to nearest even, NaN kept quiet (what cvt.rn.bf16.f32 does)
 inline uint16_t emu_f32_to_bf16(float x) {

@@ -16,6 +16,7 @@
 #include "../b2d_staged.cuh"
 #include "../b2d_owner.cuh"
 #include "../b2d_syncbn.cuh"
+#include "../b2d_clip.cuh"
 #include "../b2d_launch.cuh"
 
 thread_local EmuDim3 threadIdx, blockIdx, blockDim, gridDim;
@@ -259,9 +260,10 @@ int emu_reduce_to_owner(void* h, int bf16, int nvls, float** grads, float** redu
 
 // K13: params live in every arena at param_off; m, v, reduced are the ranks' own-shard buffers.  One Adam group per
 // rank covering [glo[r], ghi[r]) of its shard (ngroups = 0: push only).
-int emu_adam_push(void* h, int nvls, size_t param_off, float** m, float** v, float** reduced, size_t n, const long long* shard_off,
-                  int ngroups, const long long* glo, const long long* ghi, float lr, float beta1, float beta2, float eps, float wd,
-                  int step, int adamw, unsigned epoch, int order, int use_generic_w) {
+static int adam_push_impl(void* h, int nvls, size_t param_off, float** m, float** v, float** reduced, size_t n,
+                          const long long* shard_off, int ngroups, const long long* glo, const long long* ghi, float lr, float beta1,
+                          float beta2, float eps, float wd, int step, int adamw, unsigned epoch, int order, int use_generic_w,
+                          float** grad_scale) {
   Group* g = static_cast<Group*>(h);
   const int world = g->world;
   if (param_off + n * 4 > g->arena_bytes) return -4;
@@ -279,9 +281,12 @@ int emu_adam_push(void* h, int nvls, size_t param_off, float** m, float** v, flo
       P.group[0] = adam_consts(b2d_adam{lr, beta1, beta2, eps, wd, step, adamw, 0});
     }
     P.rank = r; P.world = world; P.epoch = epoch; P.peers = peers;
+    P.grad_scale = grad_scale ? grad_scale[r] : nullptr;
     auto run = [=] {
       dispatch_world(use_generic_w ? 0 : world, [&](auto w) {
-        if (nvls) adam_push_kernel<decltype(w)::value, true>(P); else adam_push_kernel<decltype(w)::value, false>(P);
+        constexpr int W = decltype(w)::value;
+        if (P.grad_scale != nullptr) { if (nvls) adam_push_scaled_kernel<W, true>(P); else adam_push_scaled_kernel<W, false>(P); }
+        else { if (nvls) adam_push_kernel<W, true>(P); else adam_push_kernel<W, false>(P); }
       });
     };
     return launch_one(2, kExThreads, run);
@@ -301,6 +306,23 @@ int emu_adam_push(void* h, int nvls, size_t param_off, float** m, float** v, flo
   for (int r = 0; r < world; ++r) streams.emplace_back([&, r] { if (X(r) != 0 || Wt(r) != 0) bad = 1; });
   for (auto& t : streams) t.join();
   return bad.load() ? -1 : 0;
+}
+
+int emu_adam_push(void* h, int nvls, size_t param_off, float** m, float** v, float** reduced, size_t n, const long long* shard_off,
+                  int ngroups, const long long* glo, const long long* ghi, float lr, float beta1, float beta2, float eps, float wd,
+                  int step, int adamw, unsigned epoch, int order, int use_generic_w) {
+  return adam_push_impl(h, nvls, param_off, m, v, reduced, n, shard_off, ngroups, glo, ghi, lr, beta1, beta2, eps, wd, step, adamw,
+                        epoch, order, use_generic_w, nullptr);
+}
+
+// K13 with the gradients multiplied by *grad_scale[r] (adam_push_scaled_kernel)
+int emu_adam_push_scaled(void* h, int nvls, size_t param_off, float** m, float** v, float** reduced, size_t n,
+                         const long long* shard_off, int ngroups, const long long* glo, const long long* ghi, float lr, float beta1,
+                         float beta2, float eps, float wd, int step, int adamw, unsigned epoch, int order, int use_generic_w,
+                         float** grad_scale) {
+  if (grad_scale == nullptr) return -1;
+  return adam_push_impl(h, nvls, param_off, m, v, reduced, n, shard_off, ngroups, glo, ghi, lr, beta1, beta2, eps, wd, step, adamw,
+                        epoch, order, use_generic_w, grad_scale);
 }
 
 // K14: one optimizer step of a bucket whose parameters (and their state tensors) are separate allocations.
@@ -478,6 +500,44 @@ int emu_bn_exchange(void* h, int fwd, int channels, const float** a, const float
   for (auto& t : streams) t.join();
   return bad.load() ? -1 : 0;
 }
+
+// K18 + K19 of one clip call, laid out as b2d.cu lays out the clip region at clip_off: [gen 0 | gen 1 | block sums].
+// x[r]: rank r's n[r] elements; norm_out[r] / coef_out[r]: one float each.  gmax: the block cap (kClipGMax in the
+// library).  order as in emu_staged_allreduce (0 / 1).
+int emu_clip_norm(void* h, const float** x, const size_t* n, float max_norm, float** norm_out, float** coef_out, size_t clip_off,
+                  int gen, unsigned gmax, unsigned epoch, int order) {
+  Group* g = static_cast<Group*>(h);
+  const int world = g->world;
+  const size_t gen_bytes = static_cast<size_t>(world) * kClipSlotBytes;
+  if (gmax < 1 || gmax > static_cast<unsigned>(kClipThreads)) return -2;
+  if (clip_off + 2 * gen_bytes + gmax * sizeof(double) > g->arena_bytes) return -4;
+  const Peers peers = make_peers(*g);
+  auto partial = [&](int r) {
+    ClipPartialParams P{};
+    P.x = x[r]; P.n = n[r]; P.vec = (reinterpret_cast<uintptr_t>(x[r]) % 16) == 0;
+    P.block_sums = reinterpret_cast<double*>(g->arena[r] + clip_off + 2 * gen_bytes);
+    P.region_off = clip_off + (gen & 1) * gen_bytes; P.rank = r; P.world = world; P.epoch = epoch; P.peers = peers;
+    return launch_one(static_cast<int>(clip_grid(n[r], gmax)), kClipThreads, [P] { sqnorm_partial_kernel(P); });
+  };
+  auto coef = [&](int r) {
+    ClipCoefParams P{};
+    P.region_off = clip_off + (gen & 1) * gen_bytes; P.max_norm = max_norm; P.norm_out = norm_out[r]; P.coef_out = coef_out[r];
+    P.rank = r; P.world = world; P.epoch = epoch; P.timeout_ns = 120ull * 1000000000ull; P.diag = nullptr; P.peers = peers;
+    return launch_one(1, 32, [P] { clip_coef_kernel(P); });
+  };
+  if (order == 1) {
+    for (int r = 0; r < world; ++r) if (partial(r) != 0) return -1;
+    for (int r = 0; r < world; ++r) if (coef(r) != 0) return -1;
+    return 0;
+  }
+  std::atomic<int> bad{0};
+  std::vector<std::thread> streams;
+  for (int r = 0; r < world; ++r) streams.emplace_back([&, r] { if (partial(r) != 0 || coef(r) != 0) bad = 1; });
+  for (auto& t : streams) t.join();
+  return bad.load() ? -1 : 0;
+}
+
+unsigned emu_clip_gmax(void) { return kClipGMax; }
 
 float* emu_arena_ptr(void* h, int rank, size_t off) {
   return reinterpret_cast<float*>(static_cast<Group*>(h)->arena[rank] + off);

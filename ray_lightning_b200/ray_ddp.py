@@ -26,6 +26,10 @@ copy.  New knobs ride in as keyword arguments prefixed ``b200_`` and never reach
                               per step, one parameter group
     b200_enable=True
 
+``Trainer(gradient_clip_val=...)`` clips the averaged gradients after DDP's backward with torch's own
+``clip_grad_norm_`` / ``clip_grad_value_`` (they are whole and identical on every rank); it cannot be combined with
+``b200_optimizer_in_backward``.
+
 ``Trainer(sync_batchnorm=True)`` on the libb2d path converts every BatchNorm to ``syncbn.B200SyncBatchNorm``, whose
 statistics cross ranks through the arena; elsewhere it is torch's ``SyncBatchNorm``.
 
@@ -223,6 +227,9 @@ class RayStrategy(DDPSpawnStrategy):
         return super().training_step(*args)
 
     def setup_optimizers(self, trainer) -> None:
+        if self._b200["optimizer_in_backward"] and (getattr(trainer, "gradient_clip_val", None) or 0) > 0:
+            raise ValueError("b200_optimizer_in_backward=True cannot be combined with gradient_clip_val: the step runs "
+                             "inside backward, before the gradient norm is known")
         super().setup_optimizers(trainer)
         st = self.b200_state
         if st is not None and self._b200["optimizer_in_backward"] and self.root_device.type == "cuda":

@@ -102,6 +102,18 @@ class RayShardedStrategy(RayStrategy, DDPSpawnShardedStrategy):
                 wrapped.append(z)
             self.optimizers = wrapped
 
+    def clip_gradients(self, optimizer, clip_val, algorithm="norm"):
+        """On the GPU the gradients exist only as every owner's shard of the averaged gradient (``param.grad`` are zero
+        by now): the ``ShardedOptimizer`` clips there, with a global norm over every rank.  On the CPU reference path DDP
+        leaves whole gradients and torch's own clipping applies."""
+        from .sharded import ShardedOptimizer
+        if not isinstance(optimizer, ShardedOptimizer):
+            return super().clip_gradients(optimizer, clip_val, algorithm)
+        if algorithm == "value":
+            optimizer.clip_grad_value(clip_val)
+        else:
+            optimizer.clip_grad_norm(clip_val)
+
     def training_step(self, *args):
         if self._shards is None:
             return super().training_step(*args)

@@ -17,7 +17,10 @@ stepping the owned shard and broadcasting it — is laid out here GPU-first:
   registers, per parameter group, new parameters pushed into every rank's flat buffer) + a one-warp wait; any
   other elementwise optimizer runs ``base.step()`` on views of the owned shard and pushes the result;
 * optimizer state exists only for the owned shard (the memory saving OSS is used for) and is consolidated to the
-  stock ``torch.optim`` state-dict layout for checkpoints, which can be loaded back at ANY world size.
+  stock ``torch.optim`` state-dict layout for checkpoints, which can be loaded back at ANY world size;
+* gradient clipping acts on the owned shards of the averaged gradient, where the gradients are by then:
+  ``clip_grad_norm`` computes the global norm on the device (b2d_clip_norm: K18 + K19) and the coefficient is applied
+  inside the fused step (or by one multiply before a generic ``base.step()``); ``clip_grad_value`` clamps the shard.
 """
 from typing import List
 
@@ -171,6 +174,9 @@ class ShardedOptimizer(torch.optim.Optimizer):
         self._discard = False
         self._pass_done = False
         self._grads_clean = True
+        self._clip_bufs = None              # (norm, coef) device scalars, once the clip region is registered
+        self._coef = None                   # the clip coefficient the next step() applies
+        self._clipped = False               # gradients have been clipped since the last step
         self._hooks = []
         if self.overlap:
             for i, p in enumerate(sh.params):
@@ -196,6 +202,9 @@ class ShardedOptimizer(torch.optim.Optimizer):
         sh = self.shards
         cur, side = self._streams()
         if b == 0:
+            if self._clipped:
+                raise RuntimeError("a backward pass started after the gradients were clipped and before optimizer.step(): "
+                                   "clip once, right before the step (or call zero_grad() first)")
             if self._backward_seen:
                 # gradient accumulation: a second backward without a step in between.  The parameter exchange that
                 # normally fences the staging regions between two uses has not happened: fence explicitly, and add.
@@ -224,12 +233,56 @@ class ShardedOptimizer(torch.optim.Optimizer):
             self._next += 1
 
     def zero_grad(self, set_to_none: bool = False):
+        self._coef, self._clipped = None, False     # a pending clip coefficient belongs to the gradients dropped here
         if self._backward_seen:
             self._discard = True      # gradients reduced since the last step are being thrown away, not accumulated
         if not self._grads_clean:
             self.shards.flat_grads.zero_()
             self._grads_clean = True
         self.shards.rebind_grads()
+
+    # ---- gradient clipping: on the averaged gradient, i.e. the owned shards ------------------------------------------
+    def _own_grads(self):
+        sh = self.shards
+        return sh.reduced[:sh.own.stop - sh.own.start]
+
+    @torch.no_grad()
+    def clip_grad_norm(self, max_norm, norm_type=2.0):
+        """Collective (every rank calls it at the same step), like FairScale's ``OSS.clip_grad_norm``: the 2-norm of the
+        whole averaged gradient over all ranks, returned as a device tensor valid on the current stream.  The gradients
+        are scaled by ``min(max_norm / (norm + 1e-6), 1)`` — torch's ``clip_grad_norm_`` — inside the next ``step()``;
+        no host synchronisation."""
+        if float(norm_type) != 2.0:
+            raise ValueError("ShardedOptimizer.clip_grad_norm supports norm_type=2 only (got %r)" % (norm_type,))
+        sh = self.shards
+        cur, side = self._streams()
+        self._flush()                  # every bucket reduced: the shard holds the whole averaged gradient
+        if self._clip_bufs is None:
+            self.comm.clip_register()  # collective point: compares the region's offset across ranks once
+            dev = sh.flat_params.device
+            self._clip_bufs = (torch.zeros(1, device=dev), torch.zeros(1, device=dev))
+        norm, coef = self._clip_bufs
+        # waits for the current stream too: the returned norm of a previous call is read there
+        self.comm.clip_norm_(self._own_grads(), max_norm, norm, coef, wait_stream=cur, comm_stream=side)
+        self._coef = coef
+        self._clipped = True
+        if side is not cur:
+            cur.wait_stream(side)
+        return norm.clone()
+
+    @torch.no_grad()
+    def clip_grad_value(self, clip_value):
+        """``clip_grad_value_`` on the averaged gradient: element-wise, so clamping every owned shard is the same."""
+        v = float(clip_value)
+        cur, side = self._streams()
+        self._flush()
+        if side is not None and side is not cur:
+            with torch.cuda.stream(side):
+                self._own_grads().clamp_(min=-v, max=v)
+            cur.wait_stream(side)
+        else:
+            self._own_grads().clamp_(min=-v, max=v)
+        self._clipped = True
 
     # ---- the step ------------------------------------------------------------------------------------------
     @torch.no_grad()
@@ -247,8 +300,9 @@ class ShardedOptimizer(torch.optim.Optimizer):
                     groups.append((lo, hi, dict(lr=float(g["lr"]), beta1=float(g["betas"][0]), beta2=float(g["betas"][1]),
                                                 eps=float(g["eps"]), weight_decay=float(g["weight_decay"]),
                                                 step=self._steps, adamw=int(self._base_cls is torch.optim.AdamW))))
+            clip = {} if self._coef is None else {"grad_scale": self._coef}
             self.comm.adam_push_(sh.flat_params, self.exp_avg, self.exp_avg_sq, sh.reduced, sh.shard_off, groups,
-                                 nvls=self.nvls, wait_stream=side, comm_stream=side)
+                                 nvls=self.nvls, wait_stream=side, comm_stream=side, **clip)
         else:
             for g, bg in zip(self.param_groups, self._base.param_groups):   # lr schedulers edit OUR groups: mirror them
                 for k, v in g.items():
@@ -256,8 +310,12 @@ class ShardedOptimizer(torch.optim.Optimizer):
                         bg[k] = v
             if side is not None:
                 with torch.cuda.stream(side):
+                    if self._coef is not None:
+                        self._own_grads().mul_(self._coef)
                     self._base.step()
             else:
+                if self._coef is not None:
+                    self._own_grads().mul_(self._coef)
                 self._base.step()
             self.comm.adam_push_(sh.flat_params, None, None, None, sh.shard_off, [], nvls=self.nvls,
                                  wait_stream=side, comm_stream=side)
@@ -269,6 +327,7 @@ class ShardedOptimizer(torch.optim.Optimizer):
         self._accumulating = False
         self._discard = False
         self._pass_done = False
+        self._coef, self._clipped = None, False
         return loss
 
     # ---- checkpoints: stock torch.optim layout (SURVEY §8 f-4) -------------------------------------
