@@ -180,14 +180,28 @@ int b2d_allreduce_bucket_phased(b2d_ctx* ctx, int bucket_idx, float* grad_inout,
                                 int wire, float scale, int algo, unsigned phases,
                                 void* wait_stream, void* comm_stream);
 
-/* Hyper-parameters of the partitioned Adam (torch/optim/adam.py:347-547 semantics,
- * non-amsgrad, non-maximize).  `step` is the 1-based step count AFTER increment. */
+/* Hyper-parameters of the partitioned Adam (torch/optim/adam.py semantics, non-amsgrad, non-maximize).  `step` is the
+ * 1-based step count AFTER increment.  The values are fp32: the library derives the kernel constants from them as if
+ * they were the Python floats, so a value that fp32 does not hold exactly (beta2 = 0.999) gives constants that differ
+ * from torch's in the last bits.  b2d_adam64 and the *64 entry points carry the Python floats themselves. */
 typedef struct b2d_adam {
   float lr, beta1, beta2, eps, weight_decay;
   int32_t step;
   int32_t adamw;      /* 0: L2 (grad += wd*p) like torch.optim.Adam; 1: decoupled like AdamW */
   int32_t zero_grads; /* 1: overwrite the local flat grads with 0 once they are staged */
 } b2d_adam;
+
+/* b2d_adam with the floating-point hyper-parameters as doubles: the Python floats themselves.  The library forms
+ * `1 - beta2`, `beta ** step`, `lr / bias_correction1`, `bias_correction2 ** 0.5` and `1 - lr * weight_decay` from them
+ * in double, as torch does, and casts each to fp32 once: the update is then bit-exact against torch.optim.Adam / AdamW
+ * on CUDA (default foreach path). */
+typedef struct b2d_adam64 {
+  double lr, beta1, beta2, eps, weight_decay;
+  int32_t step;
+  int32_t adamw;
+  int32_t zero_grads;
+  int32_t pad_;
+} b2d_adam64;
 
 /* Replaces: what RayShardedStrategy (ray_lightning/ray_ddp_sharded.py:12-13) reaches through PL's
  * DDPSpawnShardedStrategy: FairScale ShardedDataParallel's reduce-to-owner of every gradient,
@@ -205,6 +219,11 @@ int b2d_sharded_step(b2d_ctx* ctx, int slot, const float* grads, float* params,
                      float* exp_avg, float* exp_avg_sq, size_t n,
                      const int64_t* shard_off, int wire, float scale,
                      const b2d_adam* adam, void* wait_stream, void* comm_stream);
+/* b2d_sharded_step with double hyper-parameters (b2d_adam64). */
+int b2d_sharded_step64(b2d_ctx* ctx, int slot, const float* grads, float* params,
+                       float* exp_avg, float* exp_avg_sq, size_t n,
+                       const int64_t* shard_off, int wire, float scale,
+                       const b2d_adam64* adam, void* wait_stream, void* comm_stream);
 
 /* Replaces: FairScale's dist.reduce(grad, dst=owner) stream for optimizers other than Adam/AdamW.
  * K4 alone: out[0 .. len_r) = sum_r grads_r[shard_off[rank] ..) * scale  (fp32 out, local). */
@@ -254,6 +273,10 @@ typedef struct b2d_adam_group {
   b2d_adam adam;
   int32_t pad_;
 } b2d_adam_group;
+typedef struct b2d_adam_group64 {
+  int64_t lo, hi;
+  b2d_adam64 adam;
+} b2d_adam_group64;
 
 /* Replaces: OSS.step() on the owned shard + OSS._broadcast_params() (one broadcast per owner).  Applies Adam /
  * AdamW (torch/optim/adam.py:530-547 arithmetic) to the own shard using `reduced` — per parameter group — and
@@ -263,6 +286,10 @@ typedef struct b2d_adam_group {
 int b2d_adam_push(b2d_ctx* ctx, float* params, float* exp_avg, float* exp_avg_sq, const float* reduced, size_t n,
                   const int64_t* shard_off, const b2d_adam_group* groups, int ngroups, unsigned flags,
                   unsigned phases, void* wait_stream, void* comm_stream);
+/* b2d_adam_push with double hyper-parameters (b2d_adam_group64). */
+int b2d_adam_push64(b2d_ctx* ctx, float* params, float* exp_avg, float* exp_avg_sq, const float* reduced, size_t n,
+                    const int64_t* shard_off, const b2d_adam_group64* groups, int ngroups, unsigned flags,
+                    unsigned phases, void* wait_stream, void* comm_stream);
 
 /* ---- optimizer step inside backward, per DDP bucket (f-2) ----------------------------------- */
 
@@ -276,11 +303,15 @@ int b2d_optim_register(b2d_ctx* ctx, int bucket_id, float* const* params, float*
                        const int64_t* bucket_off, const int64_t* numel, int nparam);
 
 /* Apply one optimizer step to the bucket's parameters from its (already averaged) gradients `grads` on `stream`:
- * kind 0 = torch.optim.SGD (hp->lr, hp->weight_decay, `momentum`; dampening 0, no nesterov; momentum buffers
- * zero-initialised), kind 1 = torch.optim.Adam / AdamW (all of *hp).  Issue it behind b2d_allreduce_bucket on the
+ * kind 0 = torch.optim.SGD (hp->lr, hp->weight_decay, `momentum`; dampening 0, no nesterov; at hp->step <= 1 the
+ * momentum buffers are written with the gradient, as torch clones it, afterwards they are read), kind 1 =
+ * torch.optim.Adam / AdamW (all of *hp).  Issue it behind b2d_allreduce_bucket on the
  * same comm stream. */
 int b2d_bucket_optim(b2d_ctx* ctx, int bucket_id, const float* grads, size_t n, int kind, const b2d_adam* hp,
                      float momentum, void* stream);
+/* b2d_bucket_optim with double hyper-parameters (b2d_adam64); `momentum` is cast to fp32 as torch casts it. */
+int b2d_bucket_optim64(b2d_ctx* ctx, int bucket_id, const float* grads, size_t n, int kind, const b2d_adam64* hp,
+                       float momentum, void* stream);
 
 /* Replaces: nothing in the reference (dist.barrier is host side); device-side fence of this library.
  * All-ranks barrier enqueued on `stream` (also quiesces the arena before slots are re-laid out). */
@@ -320,6 +351,11 @@ int b2d_bn_grad_exchange(b2d_ctx* ctx, int layer_id, const float* sum_dy, const 
 int b2d_adam_push_scaled(b2d_ctx* ctx, float* params, float* exp_avg, float* exp_avg_sq, const float* reduced, size_t n,
                          const int64_t* shard_off, const b2d_adam_group* groups, int ngroups, unsigned flags,
                          unsigned phases, void* wait_stream, void* comm_stream, const float* grad_scale);
+/* b2d_adam_push_scaled with double hyper-parameters (b2d_adam_group64). */
+int b2d_adam_push_scaled64(b2d_ctx* ctx, float* params, float* exp_avg, float* exp_avg_sq, const float* reduced,
+                           size_t n, const int64_t* shard_off, const b2d_adam_group64* groups, int ngroups,
+                           unsigned flags, unsigned phases, void* wait_stream, void* comm_stream,
+                           const float* grad_scale);
 
 /* ---- gradient clipping (b2d_clip.cuh) ------------------------------------------------------ */
 

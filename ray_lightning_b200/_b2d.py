@@ -36,6 +36,7 @@ EXPORTED_SYMBOLS = [
     "b2d_bucket_register", "b2d_reduce_to_owner", "b2d_adam_push", "b2d_ctx_set_auto_profile",
     "b2d_optim_register", "b2d_bucket_optim", "b2d_bn_register", "b2d_bn_stats_exchange", "b2d_bn_grad_exchange",
     "b2d_adam_push_scaled", "b2d_clip_register", "b2d_clip_norm",
+    "b2d_sharded_step64", "b2d_adam_push64", "b2d_adam_push_scaled64", "b2d_bucket_optim64",
 ]
 PROFILE_OVERLAP, PROFILE_LATENCY = 0, 1
 RTO_ZERO_GRADS, RTO_ACCUMULATE, RTO_NVLS = 1, 2, 4
@@ -52,6 +53,14 @@ class B2DError(RuntimeError):
 
 
 class AdamParams(ctypes.Structure):
+    """b2d_adam64: the Python floats themselves, so that the library forms torch's constants from the same doubles."""
+    _fields_ = [("lr", ctypes.c_double), ("beta1", ctypes.c_double), ("beta2", ctypes.c_double),
+                ("eps", ctypes.c_double), ("weight_decay", ctypes.c_double), ("step", ctypes.c_int32),
+                ("adamw", ctypes.c_int32), ("zero_grads", ctypes.c_int32), ("pad_", ctypes.c_int32)]
+
+
+class AdamParams32(ctypes.Structure):
+    """b2d_adam: the fp32 form of the C ABI's first Adam entry points."""
     _fields_ = [("lr", ctypes.c_float), ("beta1", ctypes.c_float), ("beta2", ctypes.c_float),
                 ("eps", ctypes.c_float), ("weight_decay", ctypes.c_float), ("step", ctypes.c_int32),
                 ("adamw", ctypes.c_int32), ("zero_grads", ctypes.c_int32)]
@@ -62,7 +71,13 @@ class Seg(ctypes.Structure):
 
 
 class AdamGroup(ctypes.Structure):
-    _fields_ = [("lo", ctypes.c_int64), ("hi", ctypes.c_int64), ("adam", AdamParams), ("pad_", ctypes.c_int32)]
+    """b2d_adam_group64"""
+    _fields_ = [("lo", ctypes.c_int64), ("hi", ctypes.c_int64), ("adam", AdamParams)]
+
+
+class AdamGroup32(ctypes.Structure):
+    """b2d_adam_group"""
+    _fields_ = [("lo", ctypes.c_int64), ("hi", ctypes.c_int64), ("adam", AdamParams32), ("pad_", ctypes.c_int32)]
 
 
 class Stats(ctypes.Structure):
@@ -113,18 +128,26 @@ def _declare(lib):
         "b2d_ctx_set_inplace": [vp, c.c_int],
         "b2d_ctx_set_auto_profile": [vp, c.c_int],
         "b2d_optim_register": [vp, c.c_int, c.POINTER(vp), c.POINTER(vp), c.POINTER(vp), c.POINTER(c.c_int64), c.POINTER(c.c_int64), c.c_int],
-        "b2d_bucket_optim": [vp, c.c_int, vp, sz, c.c_int, c.POINTER(AdamParams), c.c_float, vp],
+        "b2d_bucket_optim": [vp, c.c_int, vp, sz, c.c_int, c.POINTER(AdamParams32), c.c_float, vp],
+        "b2d_bucket_optim64": [vp, c.c_int, vp, sz, c.c_int, c.POINTER(AdamParams), c.c_float, vp],
         "b2d_peer_bw": [vp, c.c_int, sz, c.c_int, c.c_int, c.POINTER(c.c_double)],
         "b2d_pool_bind": [vp],
         "b2d_bucket_register": [vp, c.c_int, c.POINTER(Seg), c.c_int, c.c_int],
         "b2d_reduce_to_owner": [vp, c.c_int, vp, vp, c.POINTER(c.c_int64), c.c_float, c.c_uint, c.c_uint, vp, vp],
-        "b2d_adam_push": [vp, vp, vp, vp, vp, sz, c.POINTER(c.c_int64), c.POINTER(AdamGroup), c.c_int, c.c_uint, c.c_uint, vp, vp],
+        "b2d_adam_push": [vp, vp, vp, vp, vp, sz, c.POINTER(c.c_int64), c.POINTER(AdamGroup32), c.c_int, c.c_uint, c.c_uint,
+                          vp, vp],
+        "b2d_adam_push64": [vp, vp, vp, vp, vp, sz, c.POINTER(c.c_int64), c.POINTER(AdamGroup), c.c_int, c.c_uint, c.c_uint,
+                            vp, vp],
         "b2d_sharded_step": [vp, c.c_int, vp, vp, vp, vp, sz, c.POINTER(c.c_int64), c.c_int, c.c_float,
-                             c.POINTER(AdamParams), vp, vp],
+                             c.POINTER(AdamParams32), vp, vp],
+        "b2d_sharded_step64": [vp, c.c_int, vp, vp, vp, vp, sz, c.POINTER(c.c_int64), c.c_int, c.c_float,
+                               c.POINTER(AdamParams), vp, vp],
         "b2d_reduce_scatter": [vp, c.c_int, vp, vp, sz, c.POINTER(c.c_int64), c.c_int, c.c_float, vp, vp],
         "b2d_allgather": [vp, vp, sz, c.POINTER(c.c_int64), vp, vp],
-        "b2d_adam_push_scaled": [vp, vp, vp, vp, vp, sz, c.POINTER(c.c_int64), c.POINTER(AdamGroup), c.c_int, c.c_uint,
+        "b2d_adam_push_scaled": [vp, vp, vp, vp, vp, sz, c.POINTER(c.c_int64), c.POINTER(AdamGroup32), c.c_int, c.c_uint,
                                  c.c_uint, vp, vp, vp],
+        "b2d_adam_push_scaled64": [vp, vp, vp, vp, vp, sz, c.POINTER(c.c_int64), c.POINTER(AdamGroup), c.c_int, c.c_uint,
+                                   c.c_uint, vp, vp, vp],
         "b2d_clip_register": [vp, c.POINTER(sz)],
         "b2d_clip_norm": [vp, vp, sz, c.c_float, vp, vp, c.c_uint, vp, vp],
         "b2d_bn_register": [vp, c.c_int, c.c_int, c.POINTER(sz)],
@@ -307,7 +330,7 @@ class Context:
     def sharded_step(self, slot, grads_ptr, params_ptr, m_ptr, v_ptr, n, shard_off, wire, scale, adam,
                      wait_stream, comm_stream):
         off = (ctypes.c_int64 * len(shard_off))(*[int(x) for x in shard_off])
-        self._check(self._lib.b2d_sharded_step(
+        self._check(self._lib.b2d_sharded_step64(
             self._ctx, int(slot), ctypes.c_void_p(grads_ptr), ctypes.c_void_p(params_ptr),
             ctypes.c_void_p(m_ptr), ctypes.c_void_p(v_ptr), int(n), off, int(wire), float(scale),
             ctypes.byref(adam), _stream_ptr(wait_stream), _stream_ptr(comm_stream)))
@@ -339,14 +362,14 @@ class Context:
         """groups: list of (lo, hi, AdamParams) relative to the own shard; empty: push only.  grad_scale_ptr: device fp32
         factor for the gradients (b2d_adam_push_scaled)."""
         off = (ctypes.c_int64 * len(shard_off))(*[int(x) for x in shard_off])
-        arr = (AdamGroup * max(len(groups), 1))(*[AdamGroup(int(lo), int(hi), a, 0) for lo, hi, a in groups])
+        arr = (AdamGroup * max(len(groups), 1))(*[AdamGroup(int(lo), int(hi), a) for lo, hi, a in groups])
         args = (self._ctx, ctypes.c_void_p(params_ptr), ctypes.c_void_p(m_ptr or 0), ctypes.c_void_p(v_ptr or 0),
                 ctypes.c_void_p(reduced_ptr or 0), int(n), off, arr, len(groups), int(flags), int(phases),
                 _stream_ptr(wait_stream), _stream_ptr(comm_stream))
         if grad_scale_ptr is None:
-            self._check(self._lib.b2d_adam_push(*args))
+            self._check(self._lib.b2d_adam_push64(*args))
         else:
-            self._check(self._lib.b2d_adam_push_scaled(*args, ctypes.c_void_p(grad_scale_ptr)))
+            self._check(self._lib.b2d_adam_push_scaled64(*args, ctypes.c_void_p(grad_scale_ptr)))
 
     def clip_register(self):
         """Returns the arena offset of the clip exchange's region."""
@@ -367,7 +390,7 @@ class Context:
             (ctypes.c_int64 * n)(*[int(o) for o in bucket_offs]), (ctypes.c_int64 * n)(*[int(x) for x in numels]), n))
 
     def bucket_optim(self, bucket_id, grads_ptr, n, kind, hp, momentum, stream):
-        self._check(self._lib.b2d_bucket_optim(self._ctx, int(bucket_id), ctypes.c_void_p(grads_ptr), int(n), int(kind),
+        self._check(self._lib.b2d_bucket_optim64(self._ctx, int(bucket_id), ctypes.c_void_p(grads_ptr), int(n), int(kind),
                                                ctypes.byref(hp), float(momentum), _stream_ptr(stream)))
 
     def bn_register(self, layer_id, channels):

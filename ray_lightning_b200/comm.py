@@ -701,6 +701,7 @@ class InBackwardOptimizer(torch.optim.Optimizer):
             s1, s2 = self._states(p)
             if self.kind == 0 and "momentum_buffer" in st and s1 is not None:
                 s1.copy_(st["momentum_buffer"])
+                self._steps = max(self._steps, 1)     # K14 reads the buffer instead of starting it from the gradient
             elif self.kind == 1:
                 s1.copy_(st["exp_avg"]); s2.copy_(st["exp_avg_sq"])
                 self._steps = int(st["step"])

@@ -1407,7 +1407,7 @@ int b2d_allreduce_bucket(b2d_ctx* ctx, int bucket_idx, float* grad, size_t n, in
 
 static int sharded_common(b2d_ctx* ctx, int slot, const float* grads, float* params, float* exp_avg,
                           float* exp_avg_sq, float* rs_out, size_t n, const int64_t* shard_off, int wire,
-                          float scale, const b2d_adam* adam, int do_sr, int do_gather, int end_barrier,
+                          float scale, const b2d_adam64* adam, int do_sr, int do_gather, int end_barrier,
                           void* wait_stream, void* comm_stream) {
   int rc = check_ready(ctx);
   if (rc != B2D_OK) return rc;
@@ -1470,12 +1470,21 @@ static int sharded_common(b2d_ctx* ctx, int slot, const float* grads, float* par
   return ls.end();
 }
 
+int b2d_sharded_step64(b2d_ctx* ctx, int slot, const float* grads, float* params, float* exp_avg,
+                       float* exp_avg_sq, size_t n, const int64_t* shard_off, int wire, float scale,
+                       const b2d_adam64* adam, void* wait_stream, void* comm_stream) {
+  if (adam == nullptr) return fail(ctx, B2D_ERR_INVALID, "adam is NULL");
+  return sharded_common(ctx, slot, grads, params, exp_avg, exp_avg_sq, nullptr, n, shard_off, wire, scale, adam,
+                        1, 1, 0, wait_stream, comm_stream);
+}
+
 int b2d_sharded_step(b2d_ctx* ctx, int slot, const float* grads, float* params, float* exp_avg,
                      float* exp_avg_sq, size_t n, const int64_t* shard_off, int wire, float scale,
                      const b2d_adam* adam, void* wait_stream, void* comm_stream) {
   if (adam == nullptr) return fail(ctx, B2D_ERR_INVALID, "adam is NULL");
-  return sharded_common(ctx, slot, grads, params, exp_avg, exp_avg_sq, nullptr, n, shard_off, wire, scale, adam,
-                        1, 1, 0, wait_stream, comm_stream);
+  const b2d_adam64 a = adam64(*adam);
+  return b2d_sharded_step64(ctx, slot, grads, params, exp_avg, exp_avg_sq, n, shard_off, wire, scale, &a, wait_stream,
+                            comm_stream);
 }
 
 int b2d_reduce_scatter(b2d_ctx* ctx, int slot, const float* grads, float* out, size_t n,
@@ -1581,7 +1590,7 @@ int b2d_reduce_to_owner(b2d_ctx* ctx, int bucket_id, float* grads, float* reduce
 
 // b2d_adam_push (grad_scale == NULL: K13) and b2d_adam_push_scaled (K13 with the gradients scaled on the device)
 static int adam_push(b2d_ctx* ctx, float* params, float* exp_avg, float* exp_avg_sq, const float* reduced, size_t n,
-                     const int64_t* shard_off, const b2d_adam_group* groups, int ngroups, unsigned flags, unsigned phases,
+                     const int64_t* shard_off, const b2d_adam_group64* groups, int ngroups, unsigned flags, unsigned phases,
                      void* wait_stream, void* comm_stream, const float* grad_scale) {
   int rc = check_ready(ctx);
   if (rc != B2D_OK) return rc;
@@ -1661,19 +1670,43 @@ static int adam_push(b2d_ctx* ctx, float* params, float* exp_avg, float* exp_avg
   return B2D_OK;
 }
 
+// The fp32 groups of b2d_adam_push, widened; more than kMaxAdamGroups are refused by adam_push itself.
+static std::vector<b2d_adam_group64> groups64(const b2d_adam_group* groups, int ngroups) {
+  std::vector<b2d_adam_group64> g(groups != nullptr && ngroups > 0 ? ngroups : 0);
+  for (size_t k = 0; k < g.size(); ++k) g[k] = b2d_adam_group64{groups[k].lo, groups[k].hi, adam64(groups[k].adam)};
+  return g;
+}
+
+int b2d_adam_push64(b2d_ctx* ctx, float* params, float* exp_avg, float* exp_avg_sq, const float* reduced, size_t n,
+                    const int64_t* shard_off, const b2d_adam_group64* groups, int ngroups, unsigned flags, unsigned phases,
+                    void* wait_stream, void* comm_stream) {
+  return adam_push(ctx, params, exp_avg, exp_avg_sq, reduced, n, shard_off, groups, ngroups, flags, phases, wait_stream,
+                   comm_stream, nullptr);
+}
+
+int b2d_adam_push_scaled64(b2d_ctx* ctx, float* params, float* exp_avg, float* exp_avg_sq, const float* reduced, size_t n,
+                           const int64_t* shard_off, const b2d_adam_group64* groups, int ngroups, unsigned flags,
+                           unsigned phases, void* wait_stream, void* comm_stream, const float* grad_scale) {
+  if (grad_scale == nullptr) return fail(ctx, B2D_ERR_INVALID, "grad_scale is NULL");
+  return adam_push(ctx, params, exp_avg, exp_avg_sq, reduced, n, shard_off, groups, ngroups, flags, phases, wait_stream,
+                   comm_stream, grad_scale);
+}
+
 int b2d_adam_push(b2d_ctx* ctx, float* params, float* exp_avg, float* exp_avg_sq, const float* reduced, size_t n,
                   const int64_t* shard_off, const b2d_adam_group* groups, int ngroups, unsigned flags, unsigned phases,
                   void* wait_stream, void* comm_stream) {
-  return adam_push(ctx, params, exp_avg, exp_avg_sq, reduced, n, shard_off, groups, ngroups, flags, phases, wait_stream,
-                   comm_stream, nullptr);
+  const std::vector<b2d_adam_group64> g = groups64(groups, ngroups);
+  return adam_push(ctx, params, exp_avg, exp_avg_sq, reduced, n, shard_off, groups == nullptr ? nullptr : g.data(), ngroups,
+                   flags, phases, wait_stream, comm_stream, nullptr);
 }
 
 int b2d_adam_push_scaled(b2d_ctx* ctx, float* params, float* exp_avg, float* exp_avg_sq, const float* reduced, size_t n,
                          const int64_t* shard_off, const b2d_adam_group* groups, int ngroups, unsigned flags, unsigned phases,
                          void* wait_stream, void* comm_stream, const float* grad_scale) {
   if (grad_scale == nullptr) return fail(ctx, B2D_ERR_INVALID, "grad_scale is NULL");
-  return adam_push(ctx, params, exp_avg, exp_avg_sq, reduced, n, shard_off, groups, ngroups, flags, phases, wait_stream,
-                   comm_stream, grad_scale);
+  const std::vector<b2d_adam_group64> g = groups64(groups, ngroups);
+  return adam_push(ctx, params, exp_avg, exp_avg_sq, reduced, n, shard_off, groups == nullptr ? nullptr : g.data(), ngroups,
+                   flags, phases, wait_stream, comm_stream, grad_scale);
 }
 
 // ---- gradient clipping (b2d_clip.cuh) ------------------------------------------------------------------------------
@@ -1777,6 +1810,13 @@ int b2d_optim_register(b2d_ctx* ctx, int bucket_id, float* const* params, float*
 
 int b2d_bucket_optim(b2d_ctx* ctx, int bucket_id, const float* grads, size_t n, int kind, const b2d_adam* hp, float momentum,
                      void* stream) {
+  if (hp == nullptr) return b2d_bucket_optim64(ctx, bucket_id, grads, n, kind, nullptr, momentum, stream);
+  const b2d_adam64 a = adam64(*hp);
+  return b2d_bucket_optim64(ctx, bucket_id, grads, n, kind, &a, momentum, stream);
+}
+
+int b2d_bucket_optim64(b2d_ctx* ctx, int bucket_id, const float* grads, size_t n, int kind, const b2d_adam64* hp,
+                       float momentum, void* stream) {
   if (ctx == nullptr) return fail(nullptr, B2D_ERR_INVALID, "ctx is NULL");
   std::lock_guard<std::mutex> lk(ctx->mu);
   auto it = ctx->optim_buckets.find(bucket_id);
@@ -1789,7 +1829,8 @@ int b2d_bucket_optim(b2d_ctx* ctx, int bucket_id, const float* grads, size_t n, 
   P.param_ptr = it->second.d_ptr; P.seg_start = it->second.d_start; P.nseg = it->second.nseg;
   P.state1_ptr = it->second.d_ptr + it->second.nseg; P.state2_ptr = it->second.d_ptr + 2 * it->second.nseg;
   P.grads = grads; P.n = n; P.kind = kind;
-  P.lr = hp->lr; P.momentum = momentum; P.weight_decay = hp->weight_decay;
+  P.lr = static_cast<float>(hp->lr); P.momentum = momentum; P.weight_decay = static_cast<float>(hp->weight_decay);
+  P.first_step = hp->step <= 1;
   if (kind == 1) P.adam = adam_consts(*hp);
   const int grid = clamp_grid(n, kStThreads * 4, static_cast<size_t>(ctx->sm_count) * 2);
   bucket_optim_kernel<<<grid, kStThreads, 0, static_cast<cudaStream_t>(stream)>>>(P);

@@ -403,13 +403,19 @@ __global__ void __launch_bounds__(kThreads, 1) k2_two_shot_kernel(const __grid_c
 }
 
 // ---- K4/K5/K6: sharded step ----------------------------------------------------------------
+// The fp32 kernel arguments of torch's Adam / AdamW, each one cast of Python's float64 value (adam_consts in
+// b2d_launch.cuh).
 struct AdamConsts {
-  float lr, beta1, beta2, eps, weight_decay;
-  float one_minus_beta1, one_minus_beta2;
-  float step_size;        // lr / (1 - beta1^step)
-  float inv_bc2_sqrt;     // 1 / sqrt(1 - beta2^step)
+  float beta2, eps, weight_decay;
+  float lerp_w;           // 1 - beta1, the weight of exp_avg.lerp_
+  float lerp_w_rest;      // 1 - lerp_w in fp32: the factor of lerp's second branch
+  float one_minus_beta2;
+  float neg_step_size;    // -(lr / (1 - beta1^step))
+  float bc2_sqrt;         // (1 - beta2^step) ** 0.5
   float decay_mul;        // 1 - lr * weight_decay (AdamW)
-  int adamw;
+  int lerp_small;         // |lerp_w| < 0.5: lerp's first branch
+  int l2;                 // Adam with weight_decay != 0: grad += weight_decay * param
+  int decoupled;          // AdamW with weight_decay != 0: param *= decay_mul
 };
 
 struct ShParams {
@@ -435,18 +441,22 @@ struct ShParams {
   Peers peers;
 };
 
-// torch.optim.Adam single-tensor update (torch/optim/adam.py:347-547, non-capturable branch
-// :530-547) for one element; fp32 throughout, same operation order.
+// One element of torch.optim.Adam / AdamW as torch runs it on CUDA with its default multi-tensor path
+// (torch/optim/adam.py `_multi_tensor_adam`, non-capturable): one fp32 rounding per ATen operation, in torch's order,
+// and a fused multiply-add exactly where ATen's kernel computes `a + b * c`.  Every operation is spelled out
+// (__f*_rn), so that the compiler contracts nothing else and the host build of the emulator rounds identically.
 __device__ __forceinline__ void adam_update(float g, float& p, float& m, float& v, const AdamConsts& a) {
-  if (a.adamw) {
-    p = p * a.decay_mul;                       // param.mul_(1 - lr * weight_decay)
-  } else if (a.weight_decay != 0.f) {
-    g = fmaf(a.weight_decay, p, g);            // grad = grad.add(param, alpha=weight_decay)
+  if (a.decoupled) {
+    p = __fmul_rn(p, a.decay_mul);                              // _foreach_mul_(params, 1 - lr * weight_decay)
+  } else if (a.l2) {
+    g = __fmaf_rn(a.weight_decay, p, g);                        // _foreach_add(grads, params, alpha=weight_decay)
   }
-  m = fmaf(a.one_minus_beta1, g - m, m);       // exp_avg.lerp_(grad, 1 - beta1)
-  v = fmaf(a.one_minus_beta2 * g, g, v * a.beta2);  // exp_avg_sq.mul_(beta2).addcmul_(grad, grad, 1-beta2)
-  const float denom = fmaf(sqrtf(v), a.inv_bc2_sqrt, a.eps);  // (sqrt(v) / bc2_sqrt).add_(eps)
-  p = fmaf(-a.step_size, m / denom, p);        // param.addcdiv_(exp_avg, denom, value=-step_size)
+  const float d = __fadd_rn(g, -m);                             // _foreach_lerp_(exp_avgs, grads, 1 - beta1):
+  m = a.lerp_small ? __fmaf_rn(a.lerp_w, d, m)                  //   m + w * (g - m)             for |w| < 0.5,
+                   : __fmaf_rn(-d, a.lerp_w_rest, g);           //   g - (g - m) * (1 - w)       otherwise (Lerp.h)
+  v = __fmaf_rn(a.one_minus_beta2, __fmul_rn(g, g), __fmul_rn(v, a.beta2));  // _foreach_mul_(v, beta2), _foreach_addcmul_
+  const float denom = __fadd_rn(__fdiv_rn(__fsqrt_rn(v), a.bc2_sqrt), a.eps);  // _foreach_sqrt, _foreach_div_, _foreach_add_
+  p = __fmaf_rn(a.neg_step_size, __fdiv_rn(m, denom), p);       // _foreach_addcdiv_(params, exp_avgs, denom, -step_size)
 }
 
 template <int W, bool BF16>

@@ -31,19 +31,31 @@ void dispatch_world(int world, F&& f) {
 // element count only, never on the device.  At most kClipThreads, the width of the final tree.
 constexpr unsigned kClipGMax = 256;
 
-// Python-float (double) arithmetic of torch/optim/adam.py:503-541, cast once.
-inline AdamConsts adam_consts(const b2d_adam& adam) {
+// torch/optim/adam.py's host arithmetic on Python floats (`1 - beta2`, `beta1 ** step`, `lr / bias_correction1`,
+// `bias_correction2 ** 0.5`, `1 - lr * weight_decay`) in double with the same libm pow, then one cast to fp32 each, as
+// ATen casts a Python scalar for its kernels.
+inline AdamConsts adam_consts(const b2d_adam64& adam) {
   AdamConsts a{};
-  a.lr = adam.lr; a.beta1 = adam.beta1; a.beta2 = adam.beta2; a.eps = adam.eps; a.weight_decay = adam.weight_decay;
-  a.one_minus_beta1 = static_cast<float>(1.0 - static_cast<double>(adam.beta1));
-  a.one_minus_beta2 = static_cast<float>(1.0 - static_cast<double>(adam.beta2));
-  double b1p = 1.0, b2p = 1.0;
-  for (int i = 0; i < adam.step; ++i) { b1p *= static_cast<double>(adam.beta1); b2p *= static_cast<double>(adam.beta2); }
-  a.step_size = static_cast<float>(static_cast<double>(adam.lr) / (1.0 - b1p));
-  a.inv_bc2_sqrt = 1.0f / static_cast<float>(sqrt(1.0 - b2p));
-  a.decay_mul = static_cast<float>(1.0 - static_cast<double>(adam.lr) * static_cast<double>(adam.weight_decay));
-  a.adamw = adam.adamw;
+  a.beta2 = static_cast<float>(adam.beta2);
+  a.eps = static_cast<float>(adam.eps);
+  a.weight_decay = static_cast<float>(adam.weight_decay);
+  a.lerp_w = static_cast<float>(1.0 - adam.beta1);
+  a.lerp_w_rest = 1.0f - a.lerp_w;                             // Lerp.h computes `1 - weight` in fp32
+  a.lerp_small = fabsf(a.lerp_w) < 0.5f;
+  a.one_minus_beta2 = static_cast<float>(1.0 - adam.beta2);
+  const double bc1 = 1.0 - pow(adam.beta1, static_cast<double>(adam.step));
+  const double bc2 = 1.0 - pow(adam.beta2, static_cast<double>(adam.step));
+  a.neg_step_size = static_cast<float>(adam.lr / bc1 * -1.0);
+  a.bc2_sqrt = static_cast<float>(pow(bc2, 0.5));
+  a.decay_mul = static_cast<float>(1.0 - adam.lr * adam.weight_decay);
+  a.l2 = !adam.adamw && adam.weight_decay != 0.0;
+  a.decoupled = adam.adamw && adam.weight_decay != 0.0;
   return a;
+}
+
+// The fp32 hyper-parameters of b2d_adam, widened exactly: the constants are then formed from the rounded values.
+inline b2d_adam64 adam64(const b2d_adam& a) {
+  return b2d_adam64{a.lr, a.beta1, a.beta2, a.eps, a.weight_decay, a.step, a.adamw, a.zero_grads, 0};
 }
 
 // Chunk c of a staged exchange of n elements: npacks wire packs of epp elements, chunk_packs packs per chunk.

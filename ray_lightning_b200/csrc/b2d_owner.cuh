@@ -252,8 +252,9 @@ __global__ void __launch_bounds__(kExThreads, 2) adam_push_scaled_kernel(const _
 // optimizer per parameter)).  The bucket's averaged gradients are contiguous; its parameters are separate
 // allocations, so the kernel walks a small table (first bucket element of each parameter, cumulative) and touches
 // parameters with coalesced 4-byte accesses.  Optimizer state (momentum buffer, or exp_avg / exp_avg_sq) is one
-// tensor per parameter, owned by the caller (it survives DDP's bucket re-layout).  Arithmetic follows torch.optim.SGD (sgd.py `_single_tensor_sgd`, dampening 0, no
-// nesterov) and torch.optim.Adam / AdamW (adam_update above), fp32.
+// tensor per parameter, owned by the caller (it survives DDP's bucket re-layout).  Arithmetic is torch.optim.SGD's
+// on CUDA (sgd.py, dampening 0, no nesterov; both of torch's paths issue the same element-wise operations) and
+// torch.optim.Adam / AdamW's (adam_update above), bit for bit.
 struct OptimParams {
   float* const* param_ptr;      // [nseg] device table: start of each parameter
   const unsigned* seg_start;    // [nseg + 1] first bucket element of each parameter, cumulative
@@ -264,6 +265,7 @@ struct OptimParams {
   float* const* state2_ptr;     // [nseg] unused          | exp_avg_sq
   int kind;                     // 0 SGD, 1 Adam / AdamW
   float lr, momentum, weight_decay;
+  int first_step;               // SGD: the momentum buffer starts as a copy of the gradient (torch.clone(grad))
   AdamConsts adam;
 };
 
@@ -275,14 +277,15 @@ __global__ void __launch_bounds__(kStThreads) bucket_optim_kernel(const __grid_c
     float* pp = P.param_ptr[s] + k;
     float g = P.grads[e], p = *pp;
     if (P.kind == 0) {
-      if (P.weight_decay != 0.f) g = fmaf(P.weight_decay, p, g);      // grad = grad.add(param, alpha=weight_decay)
+      if (P.weight_decay != 0.f) g = __fmaf_rn(P.weight_decay, p, g);  // grad = grad.add(param, alpha=weight_decay)
       if (P.momentum != 0.f) {
         float* bp = P.state1_ptr[s] + k;
-        const float b = __fadd_rn(__fmul_rn(P.momentum, *bp), g);      // buf.mul_(momentum).add_(grad): two roundings
+        // buf = torch.clone(grad) on the first step, then buf.mul_(momentum).add_(grad): two roundings
+        const float b = P.first_step ? g : __fadd_rn(__fmul_rn(P.momentum, *bp), g);
         *bp = b;
         g = b;
       }
-      *pp = fmaf(-P.lr, g, p);                                         // param.add_(grad, alpha=-lr)
+      *pp = __fmaf_rn(-P.lr, g, p);                                    // param.add_(grad, alpha=-lr)
     } else {
       float* mp = P.state1_ptr[s] + k;
       float* vp = P.state2_ptr[s] + k;

@@ -103,6 +103,7 @@ inline float __fmul_rn(float a, float b) { volatile float r = a * b; return r; }
 inline float __fdiv_rn(float a, float b) { volatile float r = a / b; return r; }
 inline float __fsqrt_rn(float a) { volatile float r = std::sqrt(a); return r; }
 inline float __frcp_rn(float a) { volatile float r = 1.f / a; return r; }
+inline float __fmaf_rn(float a, float b, float c) { volatile float r = std::fma(a, b, c); return r; }   // libm: one rounding
 inline double __dadd_rn(double a, double b) { volatile double r = a + b; return r; }
 inline double __dmul_rn(double a, double b) { volatile double r = a * b; return r; }
 inline double __dsqrt_rn(double a) { volatile double r = std::sqrt(a); return r; }

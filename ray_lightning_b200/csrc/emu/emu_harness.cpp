@@ -261,8 +261,8 @@ int emu_reduce_to_owner(void* h, int bf16, int nvls, float** grads, float** redu
 // K13: params live in every arena at param_off; m, v, reduced are the ranks' own-shard buffers.  One Adam group per
 // rank covering [glo[r], ghi[r]) of its shard (ngroups = 0: push only).
 static int adam_push_impl(void* h, int nvls, size_t param_off, float** m, float** v, float** reduced, size_t n,
-                          const long long* shard_off, int ngroups, const long long* glo, const long long* ghi, float lr, float beta1,
-                          float beta2, float eps, float wd, int step, int adamw, unsigned epoch, int order, int use_generic_w,
+                          const long long* shard_off, int ngroups, const long long* glo, const long long* ghi, double lr, double beta1,
+                          double beta2, double eps, double wd, int step, int adamw, unsigned epoch, int order, int use_generic_w,
                           float** grad_scale) {
   Group* g = static_cast<Group*>(h);
   const int world = g->world;
@@ -278,7 +278,7 @@ static int adam_push_impl(void* h, int nvls, size_t param_off, float** m, float*
     P.lo = shard_off[r]; P.hi = shard_off[r + 1]; P.ngroups = ngroups;
     if (ngroups > 0) {
       P.group_lo[0] = glo[r]; P.group_hi[0] = ghi[r];
-      P.group[0] = adam_consts(b2d_adam{lr, beta1, beta2, eps, wd, step, adamw, 0});
+      P.group[0] = adam_consts(b2d_adam64{lr, beta1, beta2, eps, wd, step, adamw, 0, 0});
     }
     P.rank = r; P.world = world; P.epoch = epoch; P.peers = peers;
     P.grad_scale = grad_scale ? grad_scale[r] : nullptr;
@@ -308,6 +308,14 @@ static int adam_push_impl(void* h, int nvls, size_t param_off, float** m, float*
   return bad.load() ? -1 : 0;
 }
 
+// The *64 entry points take the hyper-parameters as doubles (b2d_adam64); the others as fp32 (b2d_adam), widened.
+int emu_adam_push64(void* h, int nvls, size_t param_off, float** m, float** v, float** reduced, size_t n, const long long* shard_off,
+                    int ngroups, const long long* glo, const long long* ghi, double lr, double beta1, double beta2, double eps,
+                    double wd, int step, int adamw, unsigned epoch, int order, int use_generic_w) {
+  return adam_push_impl(h, nvls, param_off, m, v, reduced, n, shard_off, ngroups, glo, ghi, lr, beta1, beta2, eps, wd, step, adamw,
+                        epoch, order, use_generic_w, nullptr);
+}
+
 int emu_adam_push(void* h, int nvls, size_t param_off, float** m, float** v, float** reduced, size_t n, const long long* shard_off,
                   int ngroups, const long long* glo, const long long* ghi, float lr, float beta1, float beta2, float eps, float wd,
                   int step, int adamw, unsigned epoch, int order, int use_generic_w) {
@@ -316,23 +324,38 @@ int emu_adam_push(void* h, int nvls, size_t param_off, float** m, float** v, flo
 }
 
 // K13 with the gradients multiplied by *grad_scale[r] (adam_push_scaled_kernel)
-int emu_adam_push_scaled(void* h, int nvls, size_t param_off, float** m, float** v, float** reduced, size_t n,
-                         const long long* shard_off, int ngroups, const long long* glo, const long long* ghi, float lr, float beta1,
-                         float beta2, float eps, float wd, int step, int adamw, unsigned epoch, int order, int use_generic_w,
-                         float** grad_scale) {
+int emu_adam_push_scaled64(void* h, int nvls, size_t param_off, float** m, float** v, float** reduced, size_t n,
+                           const long long* shard_off, int ngroups, const long long* glo, const long long* ghi, double lr,
+                           double beta1, double beta2, double eps, double wd, int step, int adamw, unsigned epoch, int order,
+                           int use_generic_w, float** grad_scale) {
   if (grad_scale == nullptr) return -1;
   return adam_push_impl(h, nvls, param_off, m, v, reduced, n, shard_off, ngroups, glo, ghi, lr, beta1, beta2, eps, wd, step, adamw,
                         epoch, order, use_generic_w, grad_scale);
 }
 
+int emu_adam_push_scaled(void* h, int nvls, size_t param_off, float** m, float** v, float** reduced, size_t n,
+                         const long long* shard_off, int ngroups, const long long* glo, const long long* ghi, float lr, float beta1,
+                         float beta2, float eps, float wd, int step, int adamw, unsigned epoch, int order, int use_generic_w,
+                         float** grad_scale) {
+  return emu_adam_push_scaled64(h, nvls, param_off, m, v, reduced, n, shard_off, ngroups, glo, ghi, lr, beta1, beta2, eps, wd, step,
+                                adamw, epoch, order, use_generic_w, grad_scale);
+}
+
 // K14: one optimizer step of a bucket whose parameters (and their state tensors) are separate allocations.
-int emu_bucket_optim(float** params, float** state1, float** state2, const unsigned* seg_start, int nseg, const float* grads,
-                     size_t n, int kind, float lr, float momentum, float wd, float beta1, float beta2, float eps, int step, int adamw) {
+int emu_bucket_optim64(float** params, float** state1, float** state2, const unsigned* seg_start, int nseg, const float* grads,
+                       size_t n, int kind, double lr, float momentum, double wd, double beta1, double beta2, double eps, int step,
+                       int adamw) {
   OptimParams P{};
   P.param_ptr = params; P.state1_ptr = state1; P.state2_ptr = state2; P.seg_start = seg_start; P.nseg = nseg;
-  P.grads = grads; P.n = n; P.kind = kind; P.lr = lr; P.momentum = momentum; P.weight_decay = wd;
-  if (kind == 1) P.adam = adam_consts(b2d_adam{lr, beta1, beta2, eps, wd, step, adamw, 0});
+  P.grads = grads; P.n = n; P.kind = kind; P.lr = static_cast<float>(lr); P.momentum = momentum;
+  P.weight_decay = static_cast<float>(wd); P.first_step = step <= 1;
+  if (kind == 1) P.adam = adam_consts(b2d_adam64{lr, beta1, beta2, eps, wd, step, adamw, 0, 0});
   return launch_one(2, kStThreads, [P] { bucket_optim_kernel(P); });
+}
+
+int emu_bucket_optim(float** params, float** state1, float** state2, const unsigned* seg_start, int nseg, const float* grads,
+                     size_t n, int kind, float lr, float momentum, float wd, float beta1, float beta2, float eps, int step, int adamw) {
+  return emu_bucket_optim64(params, state1, state2, seg_start, nseg, grads, n, kind, lr, momentum, wd, beta1, beta2, eps, step, adamw);
 }
 
 // bufs[r]: rank r's fp32 bucket, reduced in place.  algo: 1 one-shot, 2 two-shot, 3 two-shot NVLS (fused).
@@ -374,9 +397,9 @@ int emu_k0(float* buf, size_t n, float scale, int bf16, int grid) {
 }
 
 // Fused sharded step.  params live in every arena at `param_off`; grads[r], m[r], v[r] are plain buffers.
-int emu_sharded_step(void* h, int bf16, float** grads, size_t param_off, float** m, float** v, size_t n,
-                     const long long* shard_off, float scale, float lr, float beta1, float beta2, float eps, float wd,
-                     int step, int adamw, int zero_grads, int grid, int parity, int use_generic_w) {
+int emu_sharded_step64(void* h, int bf16, float** grads, size_t param_off, float** m, float** v, size_t n,
+                       const long long* shard_off, float scale, double lr, double beta1, double beta2, double eps, double wd,
+                       int step, int adamw, int zero_grads, int grid, int parity, int use_generic_w) {
   Group* g = static_cast<Group*>(h);
   const int world = g->world;
   const size_t half = (n * (bf16 ? 2 : 4) + 255) / 256 * 256;
@@ -393,7 +416,7 @@ int emu_sharded_step(void* h, int bf16, float** grads, size_t param_off, float**
     for (int i = world + 1; i <= B2D_MAX_WORLD; ++i) P.off[i] = shard_off[world];
     P.stage_off = stage_base + (parity & 1) * half; P.scale = scale; P.rank = r; P.world = world;
     P.do_stage_reduce = 1; P.do_adam = 1; P.do_gather = 1; P.end_barrier = 0;
-    P.adam = adam_consts(b2d_adam{lr, beta1, beta2, eps, wd, step, adamw, 0});
+    P.adam = adam_consts(b2d_adam64{lr, beta1, beta2, eps, wd, step, adamw, 0, 0});
     P.timeout_ns = 60ull * 1000000000ull; P.diag = nullptr; P.peers = make_peers(*g);
     params[r] = P;
     const ShParams* pp = &params[r];
@@ -404,6 +427,13 @@ int emu_sharded_step(void* h, int bf16, float** grads, size_t param_off, float**
     });
   }
   return launch_all(world, grid, kThreads, bodies);
+}
+
+int emu_sharded_step(void* h, int bf16, float** grads, size_t param_off, float** m, float** v, size_t n,
+                     const long long* shard_off, float scale, float lr, float beta1, float beta2, float eps, float wd,
+                     int step, int adamw, int zero_grads, int grid, int parity, int use_generic_w) {
+  return emu_sharded_step64(h, bf16, grads, param_off, m, v, n, shard_off, scale, lr, beta1, beta2, eps, wd, step, adamw, zero_grads,
+                            grid, parity, use_generic_w);
 }
 
 // K4 alone (reduce-scatter to owner, fp32 out) and K6 alone (all-gather of a flat arena buffer, with its end barrier)
