@@ -55,6 +55,13 @@ def emu(tmp_path_factory):
                                        ctypes.POINTER(ctypes.c_longlong), ctypes.c_float, ctypes.c_size_t, ctypes.c_int, ctypes.c_int]
     lib.emu_allgather.argtypes = [ctypes.c_void_p, ctypes.c_size_t, ctypes.c_size_t, ctypes.POINTER(ctypes.c_longlong), ctypes.c_int]
     lib.emu_owner_table.argtypes = [LP, ctypes.c_int, ctypes.c_int, ctypes.c_int, LP, UP, UP]
+    D = ctypes.c_double
+    lib.emu_adam_push64.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_size_t, ctypes.POINTER(FP), ctypes.POINTER(FP),
+                                    ctypes.POINTER(FP), ctypes.c_size_t, LP, ctypes.c_int, LP, LP, D, D, D, D, D, ctypes.c_int,
+                                    ctypes.c_int, ctypes.c_uint, ctypes.c_int, ctypes.c_int]
+    lib.emu_sharded_step64.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.POINTER(FP), ctypes.c_size_t, ctypes.POINTER(FP),
+                                       ctypes.POINTER(FP), ctypes.c_size_t, LP, ctypes.c_float, D, D, D, D, D, ctypes.c_int,
+                                       ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int]
     lib.emu_arena_ptr.restype = FP
     lib.emu_arena_ptr.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_size_t]
     return lib
@@ -464,5 +471,356 @@ def test_owner_path_with_ranks_that_own_nothing(emu):
         for r in range(world):
             for o in range(world):
                 assert (views[r][shard_off[o]:shard_off[o + 1]] == float(o + 1)).all(), (r, o)
+    finally:
+        emu.emu_group_destroy(g)
+
+
+# ---- index math at every world size, at non-default grids, with guard bytes around every output ------------------------
+# The specialisations W = 2, 4, 8 and the generic build (W = 0: B2D_MAX_WORLD-wide arrays masked by r < world, one pack
+# per batch) cut the buckets differently; the sizes below are derived from each kernel's geometry (slices, grid-stride
+# batches, pipeline chunks) rather than listed, so that every tail a grid can meet is hit.  Every output sits between
+# two GUARD-float margins of a NaN canary (payload + a per-rank salt: a reduction of the neighbours' canaries then
+# changes some rank's margin even on the host, where NaN arithmetic keeps the first payload), compared as bits.
+CANARY = 0x7fc0beef
+GUARD = 16          # 64 bytes: a view behind the margin keeps the 16-byte alignment of its buffer
+
+
+def guarded(values, salt=0):
+    """(whole buffer, view of `values` inside it) with canary margins on both sides."""
+    values = np.asarray(values, np.float32)
+    whole = np.empty(values.size + 2 * GUARD, np.float32)
+    whole.view(np.uint32)[:] = CANARY + salt
+    whole[GUARD:GUARD + values.size] = values
+    return whole, whole[GUARD:GUARD + values.size]
+
+
+def guards_intact(whole, n, salt=0):
+    u = whole.view(np.uint32)
+    return bool((u[:GUARD] == CANARY + salt).all() and (u[GUARD + n:] == CANARY + salt).all())
+
+
+def packs_per_batch(per_pack):
+    """b2d_kernels.cuh: packs a thread handles per batch when every pack costs `per_pack` loads (W = 0: one)."""
+    return 16 // per_pack if per_pack > 0 and 16 // per_pack > 1 else 1
+
+
+def specialisation(world):
+    """b2d_launch.cuh's dispatch_world: the W a world size runs."""
+    return world if world in (2, 4, 8) else 0
+
+
+def chunk_packs(world, chunk_bytes):
+    """b2d.cu's staged_chunk_packs: the chunk in packs, rounded down to a multiple of W x 1024, at least one such unit."""
+    unit = world * 1024
+    return max(chunk_bytes // 16 // unit * unit, unit)
+
+
+def ragged(npacks, epp, i):
+    """A bucket of `npacks` packs whose last pack holds 1, epp - 1 or epp elements, by turns."""
+    return npacks * epp - (epp - 1, 1, 0)[i % 3]
+
+
+@pytest.mark.parametrize("grid", [1, 3])
+def test_k0_grid_stride_tails_and_guard_bytes(emu, grid):
+    """K0 (world 1): one grid-stride batch covers grid x 512 threads x U = 4 vectors of 4 elements; below, at and past
+    it, several batches, and the scalar tail of 1-3 elements."""
+    per_pass = grid * 512 * 4 * 4
+    for bf16 in (1, 0):
+        for k, n in enumerate((1, 2, 3, 5, per_pass - 1, per_pass, per_pass + 2, 3 * per_pass + 3)):
+            x = inputs(1, n, 40 + k)[0]
+            whole, buf = guarded(x.numpy())
+            assert emu.emu_k0(buf.ctypes.data_as(FP), n, 1.0, bf16, grid) == 0
+            want = (ddp_oracle.allreduce_bf16_wire if bf16 else ddp_oracle.allreduce_fp32_wire)([x])
+            assert same_bits(buf, want.numpy()), (grid, bf16, n)
+            assert guards_intact(whole, n), (grid, bf16, n)
+
+
+@pytest.mark.parametrize("world,grid", [(5, 1), (6, 1), (7, 1), (2, 3), (2, 5), (3, 3), (3, 5)])
+@pytest.mark.parametrize("algo", [1, 2])
+def test_allreduce_kernels_at_any_world_and_grid(emu, world, grid, algo):
+    """K1 / K2 at the world sizes only the generic build runs (5, 6, 7) and at grids of 3 and 5 blocks: fewer packs
+    than ranks (empty slices), a slice (K2) or a bucket (K1) of exactly one grid-stride batch and one pack either side
+    (k x W - 1, k x W, k x W + 1 packs), several batches; both wires, ragged last packs, guard bytes."""
+    g = emu.emu_group_create(world, 8 << 20)
+    try:
+        per_pass = grid * 512 * packs_per_batch(specialisation(world))
+        counts = sorted({1, world - 1, per_pass, per_pass + 1, world * per_pass - 1, world * per_pass, world * per_pass + 1,
+                         3 * world * per_pass + 2})
+        step = 0
+        for bf16 in (1, 0):
+            epp = 8 if bf16 else 4
+            for i, npacks in enumerate(counts):
+                n = ragged(npacks, epp, i)
+                per_rank = inputs(world, n, 500 + step)
+                held = [guarded(t.numpy(), r) for r, t in enumerate(per_rank)]
+                scale = float(np.float32(1.0) / np.float32(world))
+                assert emu.emu_allreduce(g, algo, bf16, ptrs([b for _, b in held]), n, scale, grid, step & 1, 0, 4) == 0
+                want = (ddp_oracle.allreduce_bf16_wire if bf16 else ddp_oracle.allreduce_fp32_wire)(per_rank).numpy()
+                for r, (whole, buf) in enumerate(held):
+                    assert same_bits(buf, want), (world, grid, algo, bf16, n, r)
+                    assert guards_intact(whole, n, r), (world, grid, algo, bf16, n, r)
+                step += 1
+    finally:
+        emu.emu_group_destroy(g)
+
+
+@pytest.mark.parametrize("world", [5, 6, 7])
+@pytest.mark.parametrize("nvls", [0, 1])
+def test_staged_exchange_at_any_world(emu, world, nvls):
+    """K7-K10 through the generic build with one-block stage and exchange grids: empty slices, a slice of exactly one
+    grid-stride batch of the exchange kernel and one pack past it, one chunk and one pack, and six chunks with a ragged last pack (the library's chunk of 64 KiB + 16 bytes, rounded to W x 1024 packs); the three
+    schedules of emu_staged_allreduce by turns; guard bytes around every bucket."""
+    sig = emu.emu_signal_bytes()
+    g = emu.emu_group_create(world, 16 << 20)
+    try:
+        cp = chunk_packs(world, (64 << 10) + 16)
+        per_pass = 256 * packs_per_batch(specialisation(world))
+        counts = (1, world + 1, world * per_pass, world * per_pass + 1, cp + 1, 5 * cp + world * per_pass + 3)
+        epoch, step = 1, 0
+        for bf16 in (1, 0):
+            epp = 8 if bf16 else 4
+            for i, npacks in enumerate(counts):
+                n = ragged(npacks, epp, i)
+                per_rank = inputs(world, n, 600 + 10 * step + nvls)
+                held = [guarded(t.numpy(), r) for r, t in enumerate(per_rank)]
+                scale = float(np.float32(1.0) / np.float32(world))
+                half = (step & 1) * (4 << 20)
+                rc = emu.emu_staged_allreduce(g, nvls, bf16, 0, ptrs([b for _, b in held]), n, scale, sig + half, cp, 1, 1, epoch,
+                                              step % 3, 0)
+                assert rc == 0
+                epoch += -(-npacks // cp)
+                want = (ddp_oracle.allreduce_bf16_wire if bf16 else ddp_oracle.allreduce_fp32_wire)(per_rank).numpy()
+                for r, (whole, buf) in enumerate(held):
+                    assert same_bits(buf, want), (world, nvls, bf16, n, r)
+                    assert guards_intact(whole, n, r), (world, nvls, bf16, n, r)
+                step += 1
+    finally:
+        emu.emu_group_destroy(g)
+
+
+@pytest.mark.parametrize("world", [5, 6, 7])
+@pytest.mark.parametrize("nvls", [0, 1])
+def test_staged_exchange_in_place_at_any_world_next_to_a_neighbour(emu, world, nvls):
+    """In-place fp32 buckets (n % 4 = 1, 2, 3, 0) of one to six chunks, two of them side by side in the arena with a
+    canary margin before, between and after: exchanging the second must leave the first one's result and every
+    margin alone, and the ragged last pack of each must stop at its last element."""
+    sig = emu.emu_signal_bytes()
+    g = emu.emu_group_create(world, 16 << 20)
+    try:
+        cp = chunk_packs(world, 64 << 10)
+        scale = float(np.float32(1.0) / np.float32(world))
+        epoch = 1
+        for step, (pa, pb, rag) in enumerate(((1, world - 1, 1), (cp - 1, cp + 1, 2), (5 * cp + 7, 2 * cp, 3), (3, 5 * cp + 1, 0))):
+            na, nb = pa * 4 - (4 - rag) % 4, pb * 4 - rag
+            a0 = GUARD
+            b0 = -(-(a0 + na) // 4) * 4 + GUARD
+            size = b0 + nb + GUARD
+            base = sig + 4096
+            per_a = inputs(world, na, 700 + step + 10 * nvls)
+            per_b = inputs(world, nb, 800 + step + 10 * nvls)
+            views = []
+            for r in range(world):
+                v = np.ctypeslib.as_array(emu.emu_arena_ptr(g, r, base), shape=(size,))
+                v.view(np.uint32)[:] = CANARY + r
+                v[a0:a0 + na] = per_a[r].numpy()
+                v[b0:b0 + nb] = per_b[r].numpy()
+                views.append(v)
+            for off, n in ((a0, na), (b0, nb)):
+                assert emu.emu_staged_allreduce(g, nvls, 0, 1, None, n, scale, base + 4 * off, cp, 1, 1, epoch, step % 3, 0) == 0
+                epoch += -(-(-(-n // 4)) // cp)
+            mask = np.ones(size, bool)
+            mask[a0:a0 + na] = mask[b0:b0 + nb] = False
+            for off, n, per_rank in ((a0, na, per_a), (b0, nb, per_b)):
+                want = ddp_oracle.allreduce_fp32_wire(per_rank, scale).numpy()
+                for r in range(world):
+                    got = views[r][off:off + n]
+                    if nvls and world & (world - 1):
+                        # the emulated switch adds the raw values and the kernel scales the sum (tolerance contract)
+                        np.testing.assert_allclose(got, want, rtol=1e-5, atol=1e-7)
+                        assert same_bits(got, views[0][off:off + n])
+                    else:
+                        assert same_bits(got, want), (world, nvls, n, r)
+            for r in range(world):
+                assert bool((views[r].view(np.uint32)[mask] == CANARY + r).all()), (world, nvls, step, r)
+    finally:
+        emu.emu_group_destroy(g)
+
+
+def _owner_buckets(world, kind):
+    """(numels, owner, flat offsets, shard_off, total, buckets): "empty" has W - 1 parameters, so owner W - 1 owns
+    nothing, and a first bucket holding owner 1's parameters only; "deep" has 4000 eight-element parameters and a first
+    bucket of 2000 segments that do not touch (every other parameter of each owner), so seg_find searches a deep table."""
+    if kind == "empty":
+        numels = [3001, 1203, 805, 640, 96, 51, 9][:world - 1]
+    else:
+        numels = [8] * 4000
+    owner = ddp_oracle.partition_fairscale(numels, world)
+    offs, shard_off, total = ddp_oracle.shard_layout(numels, owner, world)
+    if kind == "empty":
+        first = [i for i in range(len(numels)) if owner[i] == 1]
+    else:
+        first = [i for i in range(len(numels)) if (i // world) % 2 == 0]
+    rest = [i for i in range(len(numels)) if i not in set(first)]
+    buckets = [[(offs[i], -(-numels[i] // 8) * 8, owner[i]) for i in part] for part in (first, rest)]
+    return numels, owner, offs, shard_off, total, buckets
+
+
+@pytest.mark.parametrize("world", [5, 7])
+@pytest.mark.parametrize("kind", ["empty", "deep"])
+@pytest.mark.parametrize("bf16", [0, 1])
+def test_owner_path_at_any_world(emu, world, kind, bf16):
+    """K11 + K12 at W = 5 and 7 (generic build): an owner with an empty shard, a bucket whose segments all belong to one
+    owner (every other owner's staging range is empty), a deep segment table; then K13 (Adam + push) bit for bit
+    against torch's CUDA foreach Adam as restated in optim_ref.  Guard bytes around the gradients K11 zeroes, the
+    reduced shards K12 writes, exp_avg / exp_avg_sq and the flat parameters K13 writes; K11 must zero exactly the
+    bucket's segments, and reducing the second bucket must leave the first one's results alone."""
+    import optim_ref
+    numels, owner, offs, shard_off, total, buckets = _owner_buckets(world, kind)
+    if kind == "empty":
+        assert shard_off[world - 1] == shard_off[world]
+        assert {owner_of for _, _, owner_of in buckets[0]} == {1}
+    epp = 8 if bf16 else 4
+    sig = emu.emu_signal_bytes()
+    g = emu.emu_group_create(world, 8 << 20)
+    off = (ctypes.c_longlong * (world + 1))(*shard_off)
+    n_own = [shard_off[r + 1] - shard_off[r] for r in range(world)]
+    try:
+        scale = float(np.float32(1.0) / np.float32(world))
+        per_rank = [torch.randn(total, generator=torch.Generator().manual_seed(90 + r)) * 0.1 for r in range(world)]
+        grads = [guarded(t.numpy(), r) for r, t in enumerate(per_rank)]
+        reduced = [guarded(np.full(n, 5.0, np.float32), r) for r, n in enumerate(n_own)]
+        if bf16:
+            want = None
+            for t in per_rank:
+                c = ddp_oracle.wire_bf16(t, scale)
+                want = c if want is None else want + c
+            want = want.numpy()
+        else:
+            want = ddp_oracle.allreduce_fp32_wire(per_rank, scale).numpy()
+        done = np.zeros(total, bool)
+        epoch, wire_off = 1, sig + (1 << 20)
+        for b, segs in enumerate(buckets):
+            flat, start, opack = _seg_table(emu, segs, world, epp)
+            if kind == "deep" and b == 0:
+                assert len(flat) >= 2000
+            rc = emu.emu_reduce_to_owner(g, bf16, 0, ptrs([v for _, v in grads]), ptrs([v for _, v in reduced]), off,
+                                         (ctypes.c_longlong * len(flat))(*flat), (ctypes.c_uint * len(start))(*start), len(flat),
+                                         (ctypes.c_uint * len(opack))(*opack), wire_off, scale, 1, 0, epoch, b % 2, 0)
+            assert rc == 0
+            epoch += 1
+            wire_off += start[-1] * 16
+            for o, n, _ in segs:
+                done[o:o + n] = True
+            for r in range(world):
+                lo, hi = shard_off[r], shard_off[r + 1]
+                whole, red = reduced[r]
+                m = done[lo:hi]
+                assert same_bits(red[m], want[lo:hi][m]), (world, kind, bf16, b, r)
+                assert bool((red[~m] == 5.0).all()), (world, kind, bf16, b, r)
+                assert guards_intact(whole, hi - lo, r), (world, kind, bf16, b, r)
+                gw, gv = grads[r]
+                assert bool((gv[done] == 0.0).all()) and same_bits(gv[~done], per_rank[r].numpy()[~done]), (world, kind, b, r)
+                assert guards_intact(gw, total, r), (world, kind, bf16, b, r)
+        assert done.all()
+
+        # K13: one Adam group per owner over its whole shard, two steps, parameters pushed into every arena
+        hp = dict(lr=1e-2, beta1=0.9, beta2=0.999, eps=1e-8, weight_decay=0.01, adamw=True)
+        p = torch.randn(total, generator=torch.Generator().manual_seed(91)).numpy()
+        poff = sig + (4 << 20) + 4 * GUARD
+        views = []
+        for r in range(world):
+            v = np.ctypeslib.as_array(emu.emu_arena_ptr(g, r, poff - 4 * GUARD), shape=(total + 2 * GUARD,))
+            v.view(np.uint32)[:] = CANARY + r
+            v[GUARD:GUARD + total] = p
+            views.append(v)
+        ms = [guarded(np.zeros(n, np.float32), r) for r, n in enumerate(n_own)]
+        vs = [guarded(np.zeros(n, np.float32), r) for r, n in enumerate(n_own)]
+        gl = (ctypes.c_longlong * world)(*[0] * world)
+        gh = (ctypes.c_longlong * world)(*n_own)
+        m_ref, v_ref = np.zeros(total, np.float32), np.zeros(total, np.float32)
+        for step in (1, 2):
+            assert emu.emu_adam_push64(g, 0, poff, ptrs([x for _, x in ms]), ptrs([x for _, x in vs]), ptrs([x for _, x in reduced]),
+                                       total, off, 1, gl, gh, hp["lr"], hp["beta1"], hp["beta2"], hp["eps"], hp["weight_decay"],
+                                       step, 1, epoch, step % 2, 0) == 0
+            epoch += 1
+            p, m_ref, v_ref = optim_ref.adam_step32(p, want, m_ref, v_ref, step=step, path="foreach", **hp)
+            for r in range(world):
+                lo, hi = shard_off[r], shard_off[r + 1]
+                assert same_bits(views[r][GUARD:GUARD + total], p), (world, kind, bf16, step, r)
+                assert guards_intact(views[r], total, r), (world, kind, bf16, step, r)
+                assert same_bits(ms[r][1], m_ref[lo:hi]) and same_bits(vs[r][1], v_ref[lo:hi]), (world, kind, bf16, step, r)
+                assert guards_intact(ms[r][0], hi - lo, r) and guards_intact(vs[r][0], hi - lo, r), (world, kind, bf16, step, r)
+    finally:
+        emu.emu_group_destroy(g)
+
+
+@pytest.mark.parametrize("world,grid", [(5, 1), (7, 1), (3, 3), (2, 5)])
+@pytest.mark.parametrize("bf16", [0, 1])
+def test_sharded_step_at_any_world_and_grid(emu, world, grid, bf16):
+    """K4 + K5 + K6 (fused) and K4 alone at W = 5 and 7 with one block, and at grids of 3 and 5 blocks, with an owner
+    whose shard is empty: parameters bit for bit against optim_ref's restatement of torch's CUDA foreach Adam on the
+    oracle's reduced gradients, reduce-scatter outputs bit-exact, guard bytes around exp_avg / exp_avg_sq, the
+    reduce-scatter outputs, the gradients the step zeroes and the flat parameters."""
+    import optim_ref
+    numels = [4099, 1500, 9, 777, 2048, 3, 8200][:world - 1]
+    owner = ddp_oracle.partition_fairscale(numels, world)
+    _, shard_off, total = ddp_oracle.shard_layout(numels, owner, world)
+    n_own = [shard_off[r + 1] - shard_off[r] for r in range(world)]
+    assert 0 in n_own
+    sig = emu.emu_signal_bytes()
+    g = emu.emu_group_create(world, 8 << 20)
+    off = (ctypes.c_longlong * (world + 1))(*shard_off)
+    scale = float(np.float32(1.0) / np.float32(world))
+    try:
+        hp = dict(lr=1e-2, beta1=0.9, beta2=0.999, eps=1e-8, weight_decay=0.0, adamw=False)
+        p = torch.randn(total, generator=torch.Generator().manual_seed(12)).numpy()
+        views = []
+        for r in range(world):
+            v = np.ctypeslib.as_array(emu.emu_arena_ptr(g, r, sig), shape=(total + 2 * GUARD,))
+            v.view(np.uint32)[:] = CANARY + r
+            v[GUARD:GUARD + total] = p
+            views.append(v)
+        ms = [guarded(np.zeros(n, np.float32), r) for r, n in enumerate(n_own)]
+        vs = [guarded(np.zeros(n, np.float32), r) for r, n in enumerate(n_own)]
+        m_ref, v_ref = np.zeros(total, np.float32), np.zeros(total, np.float32)
+        for step in (1, 2):
+            per_rank = [torch.randn(total, generator=torch.Generator().manual_seed(100 * step + r)) * 0.1 for r in range(world)]
+            grads = [guarded(t.numpy(), r) for r, t in enumerate(per_rank)]
+            rc = emu.emu_sharded_step64(g, bf16, ptrs([x for _, x in grads]), sig + 4 * GUARD, ptrs([x for _, x in ms]),
+                                        ptrs([x for _, x in vs]), total, off, scale, hp["lr"], hp["beta1"], hp["beta2"], hp["eps"],
+                                        hp["weight_decay"], step, 0, 1, grid, step & 1, 0)
+            assert rc == 0
+            if bf16:
+                avg = None
+                for t in per_rank:
+                    c = ddp_oracle.wire_bf16(t, scale)
+                    avg = c if avg is None else avg + c
+                avg = avg.numpy()
+            else:
+                avg = ddp_oracle.allreduce_fp32_wire(per_rank, scale).numpy()
+            p, m_ref, v_ref = optim_ref.adam_step32(p, avg, m_ref, v_ref, step=step, path="foreach", **hp)
+            for r in range(world):
+                lo, hi = shard_off[r], shard_off[r + 1]
+                assert same_bits(views[r][GUARD:GUARD + total], p), (world, grid, bf16, step, r)
+                assert guards_intact(views[r], total, r), (world, grid, bf16, step, r)
+                assert same_bits(ms[r][1], m_ref[lo:hi]) and same_bits(vs[r][1], v_ref[lo:hi]), (world, grid, bf16, step, r)
+                assert guards_intact(ms[r][0], hi - lo, r) and guards_intact(vs[r][0], hi - lo, r), (world, grid, bf16, step, r)
+                assert bool((grads[r][1] == 0.0).all()) and guards_intact(grads[r][0], total, r), (world, grid, bf16, step, r)
+        # K4 alone into guarded outputs
+        per_rank = [torch.randn(total, generator=torch.Generator().manual_seed(300 + r)) * 0.1 for r in range(world)]
+        grads = [t.numpy().copy() for t in per_rank]
+        outs = [guarded(np.zeros(n, np.float32), r) for r, n in enumerate(n_own)]
+        assert emu.emu_reduce_scatter(g, bf16, ptrs(grads), ptrs([x for _, x in outs]), total, off, scale, sig + (2 << 20), grid, 0) == 0
+        if bf16:
+            want = None
+            for t in per_rank:
+                c = ddp_oracle.wire_bf16(t, scale)
+                want = c if want is None else want + c
+        else:
+            want = ddp_oracle.allreduce_fp32_wire(per_rank, scale)
+        for r in range(world):
+            lo, hi = shard_off[r], shard_off[r + 1]
+            assert same_bits(outs[r][1], want[lo:hi].numpy()), (world, grid, bf16, r)
+            assert guards_intact(outs[r][0], hi - lo, r), (world, grid, bf16, r)
     finally:
         emu.emu_group_destroy(g)
