@@ -14,6 +14,7 @@
 #include <algorithm>
 #include <map>
 #include <mutex>
+#include <optional>
 #include <string>
 #include <vector>
 
@@ -189,9 +190,6 @@ struct b2d_ctx {
   Diag* diag_host = nullptr;
   Diag* diag_dev = nullptr;
 
-  cudaEvent_t wait_ev[8] = {};
-  unsigned wait_ev_idx = 0;
-
   std::vector<std::pair<cudaEvent_t, cudaEvent_t>> ev_free, ev_pending;
   uint64_t launches = 0, timed_launches = 0;
   double timed_ms = 0.0;
@@ -201,9 +199,10 @@ struct b2d_ctx {
   size_t user_bottom = 0;  // user allocations grow down from the end of the arena
   std::map<size_t, size_t> slot_free;   // offset -> bytes: regions given back by re-laid-out slots (first fit)
 
-  // staged exchange (b2d_staged.cuh): three internal streams, a ring of ordering events, the chunk epoch
+  // staged exchange (b2d_staged.cuh): three internal streams, a ring of ordering events (shared by every stream
+  // join), the chunk epoch
   cudaStream_t s_stage = nullptr, s_xfer = nullptr, s_unstage = nullptr;
-  std::vector<cudaEvent_t> ev_ring;
+  std::vector<cudaEvent_t> ev_ring = std::vector<cudaEvent_t>(1024, nullptr);
   size_t ev_ring_idx = 0;
   cudaEvent_t last_unstage_ev = nullptr;   // own event, re-recorded after every write-back / parameter wait
   uint32_t epoch = 0;
@@ -374,53 +373,74 @@ bool take_timing_pair(b2d_ctx* ctx, TimingPair* out) {
   return true;
 }
 
-// `waiter` runs what is issued to it next only after everything already issued to `waited`.
-int stream_wait(b2d_ctx* ctx, cudaStream_t waiter, cudaStream_t waited) {
-  cudaEvent_t e = ctx->wait_ev[ctx->wait_ev_idx++ % 8];
-  B2D_CUDA(ctx, cudaEventRecord(e, waited));
-  B2D_CUDA(ctx, cudaStreamWaitEvent(waiter, e, 0));
-  return B2D_OK;
-}
-
-// Everything a launch needs around the kernel itself: stream dependency + optional timing.
-struct LaunchScope {
+// A span of work on one stream, timed into `pending` (ev_pending or exch_pending) when the context times its
+// launches.  The pair is taken at construction; start() and stop() record its two events.
+struct TimedSpan {
   b2d_ctx* ctx;
-  cudaStream_t comm;
+  std::vector<TimingPair>& pending;
   TimingPair ev{nullptr, nullptr};
-  bool timing = false;
-  int begin(void* wait_stream, void* comm_stream) {
-    comm = static_cast<cudaStream_t>(comm_stream);
-    cudaStream_t ws = static_cast<cudaStream_t>(wait_stream);
-    if (ws != comm) {
-      int rc = stream_wait(ctx, comm, ws);
-      if (rc != B2D_OK) return rc;
-    }
-    if ((ctx->flags & B2D_FLAG_TIMING) && take_timing_pair(ctx, &ev)) {
-      timing = true;
-      B2D_CUDA(ctx, cudaEventRecord(ev.first, comm));
-    }
+  bool timing;
+  TimedSpan(b2d_ctx* c, std::vector<TimingPair>& p)
+      : ctx(c), pending(p), timing((c->flags & B2D_FLAG_TIMING) && take_timing_pair(c, &ev)) {}
+  int start(cudaStream_t st) {
+    if (timing) B2D_CUDA(ctx, cudaEventRecord(ev.first, st));
     return B2D_OK;
   }
-  int end() {
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return fail(ctx, B2D_ERR_CUDA, "kernel launch failed: %s", cudaGetErrorString(e));
-    ctx->launches += 1;
+  int stop(cudaStream_t st) {
     if (timing) {
-      B2D_CUDA(ctx, cudaEventRecord(ev.second, comm));
-      ctx->ev_pending.push_back(ev);
+      B2D_CUDA(ctx, cudaEventRecord(ev.second, st));
+      pending.push_back(ev);
     }
     return B2D_OK;
   }
 };
 
-// The fields of a kernel's parameters that let it wait for peers: who is who, and the watchdog.
+// The next event of the ring of ordering events (b2d_ctx_create makes them).
+cudaEvent_t next_event(b2d_ctx* ctx) { return ctx->ev_ring[ctx->ev_ring_idx++ % ctx->ev_ring.size()]; }
+
+// `waiter` runs what is issued to it next only after everything already issued to `waited`.
+int join(b2d_ctx* ctx, cudaStream_t waiter, cudaStream_t waited) {
+  cudaEvent_t e = next_event(ctx);
+  B2D_CUDA(ctx, cudaEventRecord(e, waited));
+  B2D_CUDA(ctx, cudaStreamWaitEvent(waiter, e, 0));
+  return B2D_OK;
+}
+
+// Launches `kernel` and counts the launch.
+template <typename Kernel, typename... Args>
+void launch(b2d_ctx* ctx, Kernel kernel, int grid, int block, size_t smem, cudaStream_t st, const Args&... args) {
+  kernel<<<grid, block, smem, st>>>(args...);
+  ctx->launches += 1;
+}
+
+// The end of every entry point that launched: a launch that could not be enqueued is an error.
+int launch_result(b2d_ctx* ctx, const char* what = "kernel") {
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return fail(ctx, B2D_ERR_CUDA, "%s launch failed: %s", what, cudaGetErrorString(e));
+  return B2D_OK;
+}
+
+// One timed kernel on `comm` behind `wait_stream` (K0-K6), recorded as the context's last launch.
+template <typename Kernel, typename... Args>
+int launch_timed(b2d_ctx* ctx, void* wait_stream, void* comm_stream, int algo, Kernel kernel, int grid, int block,
+                 size_t smem, const Args&... args) {
+  cudaStream_t ws = static_cast<cudaStream_t>(wait_stream), comm = static_cast<cudaStream_t>(comm_stream);
+  int rc = ws != comm ? join(ctx, comm, ws) : B2D_OK;
+  if (rc != B2D_OK) return rc;
+  TimedSpan span(ctx, ctx->ev_pending);
+  rc = span.start(comm);
+  if (rc != B2D_OK) return rc;
+  launch(ctx, kernel, grid, block, smem, comm, args...);
+  ctx->last_algo = algo; ctx->last_grid = grid; ctx->last_block = kThreads;
+  rc = launch_result(ctx);
+  return rc != B2D_OK ? rc : span.stop(comm);
+}
+
+// The fields of a kernel's parameters that let it wait for peers, from the context.
 template <typename Params>
 void set_peer_wait(const b2d_ctx* ctx, Params* P) {
-  P->rank = ctx->rank;
-  P->world = ctx->world;
-  P->peers = ctx->peers;
-  P->timeout_ns = static_cast<unsigned long long>(ctx->timeout_ms) * 1000000ull;
-  P->diag = ctx->diag_dev;
+  set_peer_wait(P, ctx->rank, ctx->world, ctx->peers, static_cast<unsigned long long>(ctx->timeout_ms) * 1000000ull,
+                ctx->diag_dev);
 }
 
 // ceil(work / per_cta) CTAs, at least one, at most cap
@@ -431,11 +451,8 @@ int clamp_grid(size_t work, size_t per_cta, size_t cap) {
 int launch_barrier(b2d_ctx* ctx, cudaStream_t stream) {
   ArParams P{};
   set_peer_wait(ctx, &P);
-  barrier_kernel<<<B2D_MAX_BLOCKS, 32, 0, stream>>>(P);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return fail(ctx, B2D_ERR_CUDA, "barrier launch failed: %s", cudaGetErrorString(e));
-  ctx->launches += 1;
-  return B2D_OK;
+  launch(ctx, barrier_kernel, B2D_MAX_BLOCKS, 32, 0, stream, P);
+  return launch_result(ctx, "barrier");
 }
 
 bool is_staged(int algo) { return algo == B2D_ALGO_STAGED || algo == B2D_ALGO_NVLS; }
@@ -514,16 +531,6 @@ int pick_grid(b2d_ctx* ctx, size_t n, int wire, int algo) {
   return clamp_grid(work, kThreads, ctx->max_ctas);
 }
 
-// ---- ordering events of the staged exchange ----------------------------------------------------------------
-cudaEvent_t next_event(b2d_ctx* ctx) {
-  if (ctx->ev_ring.empty()) {
-    ctx->ev_ring.resize(1024, nullptr);
-    for (auto& e : ctx->ev_ring)
-      if (cudaEventCreateWithFlags(&e, cudaEventDisableTiming) != cudaSuccess) { cudaGetLastError(); e = nullptr; }
-  }
-  return ctx->ev_ring[ctx->ev_ring_idx++ % ctx->ev_ring.size()];
-}
-
 int ensure_streams(b2d_ctx* ctx) {
   if (ctx->s_stage != nullptr) return B2D_OK;
   int lo = 0, hi = 0;   // "greatest" priority is the numerically lowest
@@ -540,9 +547,8 @@ int ensure_streams(b2d_ctx* ctx) {
 // The final join of the internal streams: `comm` waits for everything issued to s_unstage, and last_unstage_ev marks
 // that point for get_slot's drain.
 int join_unstage(b2d_ctx* ctx, cudaStream_t comm) {
-  cudaEvent_t ed = next_event(ctx);
-  B2D_CUDA(ctx, cudaEventRecord(ed, ctx->s_unstage));
-  B2D_CUDA(ctx, cudaStreamWaitEvent(comm, ed, 0));
+  int rc = join(ctx, comm, ctx->s_unstage);
+  if (rc != B2D_OK) return rc;
   if (ctx->last_unstage_ev == nullptr) B2D_CUDA(ctx, cudaEventCreateWithFlags(&ctx->last_unstage_ev, cudaEventDisableTiming));
   B2D_CUDA(ctx, cudaEventRecord(ctx->last_unstage_ev, ctx->s_unstage));
   return B2D_OK;
@@ -631,93 +637,44 @@ int get_slot(b2d_ctx* ctx, int key, size_t half_bytes, size_t n, int wire, int a
   return B2D_OK;
 }
 
-template <bool BF16, bool NVLS>
-void launch_two_shot(const ArParams& P, int world, int grid, cudaStream_t st) {
-  dispatch_world(world, [&](auto w) { k2_two_shot_kernel<decltype(w)::value, BF16, NVLS><<<grid, kThreads, 0, st>>>(P); });
-}
-template <bool BF16>
-void launch_one_shot(const ArParams& P, int world, int grid, cudaStream_t st) {
-  dispatch_world(world, [&](auto w) { k1_one_shot_kernel<decltype(w)::value, BF16><<<grid, kThreads, 0, st>>>(P); });
-}
-template <bool BF16>
-void launch_sharded(const ShParams& P, int world, int grid, cudaStream_t st) {
-  dispatch_world(world, [&](auto w) { k456_sharded_kernel<decltype(w)::value, BF16><<<grid, kThreads, 0, st>>>(P); });
+// K2T's selector (b2d_launch.cuh holds the others; the emulator does not compile b2d_tma.cuh)
+auto select_k2t(int world) {
+  return dispatch_world(world, [](auto w) { return &k2t_two_shot_tma_kernel<decltype(w)::value, true>; });
 }
 
 // CUDA loads kernels lazily; a load can serialise against running work, and these kernels spin on
-// peers.  Load every instantiation up front (what NCCL does at communicator init).
+// peers.  Load every kernel a selector can return up front (what NCCL does at communicator init).
 template <typename K>
 void preload_one(K kernel) {
   cudaFuncAttributes a;
   if (cudaFuncGetAttributes(&a, kernel) != cudaSuccess) cudaGetLastError();
 }
-// one list per kernel family; `w` is a dispatch_world specialisation
-const auto preload_world = [](auto w) {
-  constexpr int W = decltype(w)::value;
-  preload_one(k1_one_shot_kernel<W, true>);
-  preload_one(k1_one_shot_kernel<W, false>);
-  preload_one(k2_two_shot_kernel<W, true, false>);
-  preload_one(k2_two_shot_kernel<W, false, false>);
-  preload_one(k2_two_shot_kernel<W, true, true>);
-  preload_one(k2_two_shot_kernel<W, false, true>);
-  preload_one(k2t_two_shot_tma_kernel<W, true>);
-  preload_one(k456_sharded_kernel<W, true>);
-  preload_one(k456_sharded_kernel<W, false>);
-};
-const auto preload_staged = [](auto w) {
-  constexpr int W = decltype(w)::value;
-  preload_one(exch_kernel<W, true, false, false>);
-  preload_one(exch_kernel<W, true, true, false>);
-  preload_one(exch_kernel<W, false, false, false>);
-  preload_one(exch_kernel<W, false, true, false>);
-  preload_one(exch_kernel<W, false, false, true>);
-  preload_one(exch_kernel<W, false, true, true>);
-};
-const auto preload_owner = [](auto w) {
-  constexpr int W = decltype(w)::value;
-  preload_one(seg_reduce_kernel<W, true, false>); preload_one(seg_reduce_kernel<W, true, true>);
-  preload_one(seg_reduce_kernel<W, false, false>); preload_one(seg_reduce_kernel<W, false, true>);
-  preload_one(adam_push_kernel<W, false>); preload_one(adam_push_kernel<W, true>);
-  preload_one(adam_push_scaled_kernel<W, false>); preload_one(adam_push_scaled_kernel<W, true>);
-};
-const auto tma_attr = [](auto w) {
-  if (cudaFuncSetAttribute(k2t_two_shot_tma_kernel<decltype(w)::value, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kTmaSmemBytes) != cudaSuccess)
-    cudaGetLastError();
-};
 void preload_kernels() {
-  const int worlds[] = {0, 2, 4, 8};
-  for (int world : worlds) dispatch_world(world, tma_attr);
-  for (int world : worlds) dispatch_world(world, preload_staged);
-  preload_one(stage_kernel<true>); preload_one(stage_kernel<false>);
-  preload_one(unstage_kernel<true>); preload_one(unstage_kernel<false>);
-  preload_one(arrive_kernel); preload_one(wait_published_kernel); preload_one(peer_read_kernel);
-  preload_one(seg_stage_kernel<true>); preload_one(seg_stage_kernel<false>);
-  for (int world : worlds) dispatch_world(world, preload_owner);
-  preload_one(bucket_optim_kernel);
-  preload_one(bn_push_kernel); preload_one(bn_combine_kernel<true>); preload_one(bn_combine_kernel<false>);
-  preload_one(sqnorm_partial_kernel); preload_one(clip_coef_kernel);
-  preload_one(k0_cast_scale_kernel<true>);
-  preload_one(k0_cast_scale_kernel<false>);
-  preload_one(barrier_kernel);
-  for (int world : worlds) dispatch_world(world, preload_world);
-}
-
-template <bool BF16, bool NVLS, bool INPLACE>
-void launch_exch_w(const ExParams& P, int world, int grid, cudaStream_t st) {
-  dispatch_world(world, [&](auto w) { exch_kernel<decltype(w)::value, BF16, NVLS, INPLACE><<<grid, kExThreads, 0, st>>>(P); });
-}
-template <bool BF16, bool NVLS>
-void launch_seg_reduce(const SegParams& P, int world, int grid, cudaStream_t st) {
-  dispatch_world(world, [&](auto w) { seg_reduce_kernel<decltype(w)::value, BF16, NVLS><<<grid, kExThreads, 0, st>>>(P); });
-}
-void launch_exch(const ExParams& P, int world, int grid, bool bf16, bool nvls, bool inplace, cudaStream_t st) {
-  if (inplace) {
-    if (nvls) launch_exch_w<false, true, true>(P, world, grid, st); else launch_exch_w<false, false, true>(P, world, grid, st);
-  } else if (bf16) {
-    if (nvls) launch_exch_w<true, true, false>(P, world, grid, st); else launch_exch_w<true, false, false>(P, world, grid, st);
-  } else {
-    if (nvls) launch_exch_w<false, true, false>(P, world, grid, st); else launch_exch_w<false, false, false>(P, world, grid, st);
+  for (int w : {0, 2, 4, 8}) {
+    if (cudaFuncSetAttribute(select_k2t(w), cudaFuncAttributeMaxDynamicSharedMemorySize, kTmaSmemBytes) != cudaSuccess)
+      cudaGetLastError();
+    preload_one(select_k2t(w));
+    for (bool a : {false, true}) {
+      preload_one(select_k1(w, a));
+      preload_one(select_k456(w, a));
+      for (bool b : {false, true}) {
+        preload_one(select_k2(w, a, b));
+        preload_one(select_seg_reduce(w, a, b));
+        preload_one(select_adam_push(w, a, b));
+        for (bool c : {false, true})
+          if (!(a && c)) preload_one(select_exch(w, a, b, c));   // bf16 in place is the fp32 in-place kernel
+      }
+    }
   }
+  for (bool a : {false, true}) {
+    preload_one(select_k0(a));
+    preload_one(select_stage(a));
+    preload_one(select_unstage(a));
+    preload_one(select_seg_stage(a));
+    preload_one(select_bn_combine(a));
+  }
+  preload_one(barrier_kernel); preload_one(arrive_kernel); preload_one(wait_published_kernel); preload_one(peer_read_kernel);
+  preload_one(bucket_optim_kernel); preload_one(bn_push_kernel); preload_one(sqnorm_partial_kernel); preload_one(clip_coef_kernel);
 }
 
 // The staged exchange of one bucket (b2d_staged.cuh): S on s_stage, X on s_xfer, W+U on s_unstage, chunk by
@@ -768,13 +725,12 @@ int launch_staged(b2d_ctx* ctx, int key, float* grad, size_t n, int wire, float 
 
   std::vector<cudaEvent_t> ev_s(nchunks, nullptr), ev_x(nchunks, nullptr);
   if (phases & 1u) {
-    rc = stream_wait(ctx, ctx->s_stage, wait_s);
+    rc = join(ctx, ctx->s_stage, wait_s);
     if (rc != B2D_OK) return rc;
     if (!inplace && slot->reuse_ev[half] != nullptr) B2D_CUDA(ctx, cudaStreamWaitEvent(ctx->s_stage, slot->reuse_ev[half], 0));
     if (inplace) {
       SP.epoch = epoch0 + static_cast<uint32_t>(nchunks) - 1u;   // the whole bucket is ready at once
-      arrive_kernel<<<1, 32, 0, ctx->s_stage>>>(SP);
-      ctx->launches += 1;
+      launch(ctx, arrive_kernel, 1, 32, 0, ctx->s_stage, SP);
       cudaEvent_t es = next_event(ctx);
       B2D_CUDA(ctx, cudaEventRecord(es, ctx->s_stage));
       for (int c = 0; c < nchunks; ++c) ev_s[c] = es;
@@ -785,53 +741,44 @@ int launch_staged(b2d_ctx* ctx, int key, float* grad, size_t n, int wire, float 
         SP.n = cs.n;
         SP.wire = reinterpret_cast<uint4*>(ctx->arena + stage_off) + cs.p0;
         SP.epoch = epoch0 + static_cast<uint32_t>(c);
-        const int grid = stream_grid(ctx, cs.packs);
-        if (bf16) stage_kernel<true><<<grid, kStThreads, 0, ctx->s_stage>>>(SP); else stage_kernel<false><<<grid, kStThreads, 0, ctx->s_stage>>>(SP);
-        ctx->launches += 1;
+        launch(ctx, select_stage(bf16), stream_grid(ctx, cs.packs), kStThreads, 0, ctx->s_stage, SP);
         ev_s[c] = next_event(ctx);
         B2D_CUDA(ctx, cudaEventRecord(ev_s[c], ctx->s_stage));
       }
     }
   }
   if (phases & 2u) {
-    TimingPair tp{nullptr, nullptr};
-    const bool timing = (ctx->flags & B2D_FLAG_TIMING) && take_timing_pair(ctx, &tp);
+    TimedSpan span(ctx, ctx->exch_pending);   // one pair around all the chunks
     for (int c = 0; c < nchunks; ++c) {
       const ChunkSpan cs = chunk_span(c, npacks, cp, n, epp);
       if (ev_s[c] != nullptr && (c == 0 || ev_s[c] != ev_s[c - 1])) B2D_CUDA(ctx, cudaStreamWaitEvent(ctx->s_xfer, ev_s[c], 0));
-      if (timing && c == 0) B2D_CUDA(ctx, cudaEventRecord(tp.first, ctx->s_xfer));
+      if (c == 0 && (rc = span.start(ctx->s_xfer)) != B2D_OK) return rc;
       XP.wire_off = stage_off + cs.p0 * 16;
       XP.npacks = cs.packs;
       XP.n_valid = inplace ? cs.n_valid : 0;
       XP.epoch = epoch0 + static_cast<uint32_t>(c);
       const int grid = exch_grid(ctx, cs.packs, algo);
-      launch_exch(XP, ctx->world, grid, bf16, nvls, inplace, ctx->s_xfer);
-      ctx->launches += 1;
+      launch(ctx, select_exch(ctx->world, bf16, nvls, inplace), grid, kExThreads, 0, ctx->s_xfer, XP);
       ctx->exch_launches += 1;
       ctx->last_grid = grid;
       ev_x[c] = next_event(ctx);
       B2D_CUDA(ctx, cudaEventRecord(ev_x[c], ctx->s_xfer));
     }
-    if (timing) {
-      B2D_CUDA(ctx, cudaEventRecord(tp.second, ctx->s_xfer));
-      ctx->exch_pending.push_back(tp);
-    }
+    rc = span.stop(ctx->s_xfer);
+    if (rc != B2D_OK) return rc;
   }
   if (phases & 4u) {
     for (int c = 0; c < nchunks; ++c) {
       if (ev_x[c] != nullptr) B2D_CUDA(ctx, cudaStreamWaitEvent(ctx->s_unstage, ev_x[c], 0));
       XP.epoch = epoch0 + static_cast<uint32_t>(c);
-      wait_published_kernel<<<1, 32, 0, ctx->s_unstage>>>(XP);
-      ctx->launches += 1;
+      launch(ctx, wait_published_kernel, 1, 32, 0, ctx->s_unstage, XP);
       if (!inplace) {
         const ChunkSpan cs = chunk_span(c, npacks, cp, n, epp);
         SP.grad = grad + cs.p0 * epp;
         SP.n = cs.n;
         SP.wire = reinterpret_cast<uint4*>(ctx->arena + stage_off) + cs.p0;
         SP.epoch = epoch0 + static_cast<uint32_t>(c);
-        const int grid = stream_grid(ctx, cs.packs);
-        if (bf16) unstage_kernel<true><<<grid, kStThreads, 0, ctx->s_unstage>>>(SP); else unstage_kernel<false><<<grid, kStThreads, 0, ctx->s_unstage>>>(SP);
-        ctx->launches += 1;
+        launch(ctx, select_unstage(bf16), stream_grid(ctx, cs.packs), kStThreads, 0, ctx->s_unstage, SP);
       }
     }
     rc = join_unstage(ctx, comm);
@@ -842,8 +789,8 @@ int launch_staged(b2d_ctx* ctx, int key, float* grad, size_t n, int wire, float 
     }
     slot->op_epoch0 = 0;
   }
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return fail(ctx, B2D_ERR_CUDA, "kernel launch failed: %s", cudaGetErrorString(e));
+  rc = launch_result(ctx);
+  if (rc != B2D_OK) return rc;
   ctx->last_algo = algo; ctx->last_block = kExThreads;
   return B2D_OK;
 }
@@ -897,6 +844,24 @@ int check_ready(b2d_ctx* ctx) {
                 ctx->diag_host->expect, ctx->diag_host->got);
   return B2D_OK;
 }
+
+// The way into an entry point: check_ready (`ready`) or only a NULL check, then the context's lock.  use_device()
+// switches to the context's device until the entry point returns; an entry point that allocates or launches calls it
+// after its argument checks.
+struct Entry {
+  b2d_ctx* ctx;
+  int rc;
+  std::unique_lock<std::mutex> lk;
+  std::optional<DeviceGuard> guard;
+  Entry(b2d_ctx* c, bool ready)
+      : ctx(c), rc(ready ? check_ready(c) : c == nullptr ? fail(nullptr, B2D_ERR_INVALID, "ctx is NULL") : B2D_OK) {
+    if (rc == B2D_OK) lk = std::unique_lock<std::mutex>(c->mu);
+  }
+  int use_device() {
+    guard.emplace(ctx->device);
+    return guard->ok ? B2D_OK : fail(ctx, B2D_ERR_CUDA, "cudaSetDevice(%d) failed", ctx->device);
+  }
+};
 
 }  // namespace
 
@@ -994,7 +959,7 @@ int b2d_ctx_create(int rank, int world, int device, size_t arena_bytes, unsigned
       cudaGetLastError();
     }
   }
-  for (auto& e : ctx->wait_ev) {
+  for (auto& e : ctx->ev_ring) {
     cudaError_t r = cudaEventCreateWithFlags(&e, cudaEventDisableTiming);
     if (r != cudaSuccess) { cudaGetLastError(); return bail(fail(ctx, B2D_ERR_CUDA, "cudaEventCreate failed: %s", cudaGetErrorString(r))); }
   }
@@ -1183,7 +1148,6 @@ int b2d_ctx_destroy(b2d_ctx* ctx) {
     cudaGetLastError();
     for (auto& pr : ctx->ev_pending) { cudaEventDestroy(pr.first); cudaEventDestroy(pr.second); }
     for (auto& pr : ctx->ev_free) { cudaEventDestroy(pr.first); cudaEventDestroy(pr.second); }
-    for (auto& e : ctx->wait_ev) if (e != nullptr) cudaEventDestroy(e);
     for (auto& pr : ctx->exch_pending) { cudaEventDestroy(pr.first); cudaEventDestroy(pr.second); }
     for (auto& kv : ctx->owner_buckets) free_tables(kv.second);
     for (auto& kv : ctx->optim_buckets) free_tables(kv.second);
@@ -1273,9 +1237,10 @@ int b2d_ctx_set_nvls_auto(b2d_ctx* ctx, int enable) {
 }
 
 int b2d_ctx_trace(b2d_ctx* ctx, int enable, double* phase_us, int* n_phases) {
-  if (ctx == nullptr) return fail(nullptr, B2D_ERR_INVALID, "ctx is NULL");
-  std::lock_guard<std::mutex> lk(ctx->mu);
-  DeviceGuard guard(ctx->device);
+  Entry en(ctx, false);
+  if (en.rc != B2D_OK) return en.rc;
+  int rc = en.use_device();
+  if (rc != B2D_OK) return rc;
   if (enable && ctx->trace_dev == nullptr) {
     void* p = nullptr;
     B2D_CUDA(ctx, cudaMalloc(&p, sizeof(unsigned long long) * B2D_MAX_BLOCKS * kTraceSlots));
@@ -1329,9 +1294,8 @@ int b2d_plan(b2d_ctx* ctx, size_t n, int wire, int algo, int* algo_out, int* gri
 // ---- data path ---------------------------------------------------------------------------
 int b2d_allreduce_bucket_phased(b2d_ctx* ctx, int bucket_idx, float* grad, size_t n, int wire, float scale,
                                 int algo, unsigned phases, void* wait_stream, void* comm_stream) {
-  int rc = check_ready(ctx);
-  if (rc != B2D_OK) return rc;
-  std::lock_guard<std::mutex> lk(ctx->mu);
+  Entry en(ctx, true);
+  if (en.rc != B2D_OK) return en.rc;
   if (grad == nullptr && n != 0) return fail(ctx, B2D_ERR_INVALID, "grad is NULL");
   if (reinterpret_cast<uintptr_t>(grad) % 16 != 0) return fail(ctx, B2D_ERR_INVALID, "bucket buffer must be 16-byte aligned");
   if (wire != B2D_WIRE_FP32 && wire != B2D_WIRE_BF16) return fail(ctx, B2D_ERR_INVALID, "bad wire %d", wire);
@@ -1340,8 +1304,8 @@ int b2d_allreduce_bucket_phased(b2d_ctx* ctx, int bucket_idx, float* grad, size_
     return fail(ctx, B2D_ERR_UNSUPPORTED, "NVLS requested but no multicast object is bound");
   if (phases == 0 || phases > 7u) return fail(ctx, B2D_ERR_INVALID, "bad phase mask %u", phases);
   if (n == 0) return B2D_OK;  // empty bucket: nothing to exchange, and every rank agrees on that
-  DeviceGuard guard(ctx->device);
-  if (!guard.ok) return fail(ctx, B2D_ERR_CUDA, "cudaSetDevice(%d) failed", ctx->device);
+  int rc = en.use_device();
+  if (rc != B2D_OK) return rc;
   cudaStream_t comm = static_cast<cudaStream_t>(comm_stream);
 
   int a = 0, grid = 0;
@@ -1351,15 +1315,9 @@ int b2d_allreduce_bucket_phased(b2d_ctx* ctx, int bucket_idx, float* grad, size_
     return launch_staged(ctx, bucket_idx, grad, n, wire, scale, a, phases, static_cast<cudaStream_t>(wait_stream), comm);
   if (phases != 7u) return fail(ctx, B2D_ERR_INVALID, "only the staged algorithms can be issued phase by phase");
 
-  if (ctx->world == 1) {
-    LaunchScope ls{ctx};
-    rc = ls.begin(wait_stream, comm_stream);
-    if (rc != B2D_OK) return rc;
-    if (wire == B2D_WIRE_BF16) k0_cast_scale_kernel<true><<<grid, kThreads, 0, comm>>>(grad, n, scale);
-    else k0_cast_scale_kernel<false><<<grid, kThreads, 0, comm>>>(grad, n, scale);
-    ctx->last_algo = 0; ctx->last_grid = grid; ctx->last_block = kThreads;
-    return ls.end();
-  }
+  const bool bf = wire == B2D_WIRE_BF16;
+  if (ctx->world == 1)
+    return launch_timed(ctx, wait_stream, comm_stream, 0, select_k0(bf), grid, kThreads, 0, grad, n, scale);
 
   const size_t epp = wire == B2D_WIRE_BF16 ? 8 : 4;
   const size_t npacks = (n + epp - 1) / epp;
@@ -1374,30 +1332,14 @@ int b2d_allreduce_bucket_phased(b2d_ctx* ctx, int bucket_idx, float* grad, size_
   P.grad = grad; P.n = n; P.stage_off = stage_off; P.scale = scale;
   P.trace = ctx->trace_dev;
   ctx->trace_grid = grid;
-  LaunchScope ls{ctx};
-  rc = ls.begin(wait_stream, comm_stream);
-  if (rc != B2D_OK) return rc;
-  const bool bf = wire == B2D_WIRE_BF16;
-  switch (a) {
-    case B2D_ALGO_ONE_SHOT:
-      if (bf) launch_one_shot<true>(P, ctx->world, grid, comm); else launch_one_shot<false>(P, ctx->world, grid, comm);
-      break;
-    case B2D_ALGO_TWO_SHOT:
-      if (bf) launch_two_shot<true, false>(P, ctx->world, grid, comm); else launch_two_shot<false, false>(P, ctx->world, grid, comm);
-      break;
-    case B2D_ALGO_NVLS_FUSED:
-      if (bf) launch_two_shot<true, true>(P, ctx->world, grid, comm); else launch_two_shot<false, true>(P, ctx->world, grid, comm);
-      break;
-    case B2D_ALGO_TWO_SHOT_TMA: {
-      const int mt = tma_mt(slice, grid);
-      dispatch_world(ctx->world, [&](auto w) { k2t_two_shot_tma_kernel<decltype(w)::value, true><<<grid, kTmaThreads, kTmaSmemBytes, comm>>>(P, mt); });
-      break;
-    }
-    default:
-      return fail(ctx, B2D_ERR_INVALID, "bad algo %d", a);
-  }
-  ctx->last_algo = a; ctx->last_grid = grid; ctx->last_block = kThreads;
-  return ls.end();
+  // the remaining algorithms: B2D_ALGO_ONE_SHOT, B2D_ALGO_TWO_SHOT, B2D_ALGO_NVLS_FUSED, B2D_ALGO_TWO_SHOT_TMA
+  if (a == B2D_ALGO_TWO_SHOT_TMA)
+    return launch_timed(ctx, wait_stream, comm_stream, a, select_k2t(ctx->world), grid, kTmaThreads, kTmaSmemBytes, P,
+                        tma_mt(slice, grid));
+  if (a == B2D_ALGO_ONE_SHOT)
+    return launch_timed(ctx, wait_stream, comm_stream, a, select_k1(ctx->world, bf), grid, kThreads, 0, P);
+  return launch_timed(ctx, wait_stream, comm_stream, a, select_k2(ctx->world, bf, a == B2D_ALGO_NVLS_FUSED), grid, kThreads,
+                      0, P);
 }
 
 int b2d_allreduce_bucket(b2d_ctx* ctx, int bucket_idx, float* grad, size_t n, int wire, float scale,
@@ -1409,17 +1351,16 @@ static int sharded_common(b2d_ctx* ctx, int slot, const float* grads, float* par
                           float* exp_avg_sq, float* rs_out, size_t n, const int64_t* shard_off, int wire,
                           float scale, const b2d_adam64* adam, int do_sr, int do_gather, int end_barrier,
                           void* wait_stream, void* comm_stream) {
-  int rc = check_ready(ctx);
-  if (rc != B2D_OK) return rc;
-  std::lock_guard<std::mutex> lk(ctx->mu);
+  Entry en(ctx, true);
+  if (en.rc != B2D_OK) return en.rc;
   if (shard_off == nullptr) return fail(ctx, B2D_ERR_INVALID, "shard_off is NULL");
   if (wire != B2D_WIRE_FP32 && wire != B2D_WIRE_BF16) return fail(ctx, B2D_ERR_INVALID, "bad wire %d", wire);
   size_t max_len = 0;
-  rc = check_shard_off(ctx, shard_off, n, &max_len);
+  int rc = check_shard_off(ctx, shard_off, n, &max_len);
   if (rc != B2D_OK) return rc;
   if (n == 0) return B2D_OK;
-  DeviceGuard guard(ctx->device);
-  if (!guard.ok) return fail(ctx, B2D_ERR_CUDA, "cudaSetDevice(%d) failed", ctx->device);
+  rc = en.use_device();
+  if (rc != B2D_OK) return rc;
   cudaStream_t comm = static_cast<cudaStream_t>(comm_stream);
 
   ShParams P{};
@@ -1452,22 +1393,12 @@ static int sharded_common(b2d_ctx* ctx, int slot, const float* grads, float* par
     rc = get_slot(ctx, 0x40000000 + slot, half, n, wire, 100 + do_gather, grid, comm, &stage_off);
     if (rc != B2D_OK) return rc;
     P.stage_off = stage_off;
-    LaunchScope ls{ctx};
-    rc = ls.begin(wait_stream, comm_stream);
-    if (rc != B2D_OK) return rc;
-    if (wire == B2D_WIRE_BF16) launch_sharded<true>(P, ctx->world, grid, comm);
-    else launch_sharded<false>(P, ctx->world, grid, comm);
-    ctx->last_algo = 10; ctx->last_grid = grid; ctx->last_block = kThreads;
-    return ls.end();
+    return launch_timed(ctx, wait_stream, comm_stream, 10, select_k456(ctx->world, wire == B2D_WIRE_BF16), grid, kThreads,
+                        0, P);
   }
   // all-gather only
   const int grid = clamp_grid(max_len / 4, kThreads, ctx->max_ctas);
-  LaunchScope ls{ctx};
-  rc = ls.begin(wait_stream, comm_stream);
-  if (rc != B2D_OK) return rc;
-  launch_sharded<false>(P, ctx->world, grid, comm);
-  ctx->last_algo = 11; ctx->last_grid = grid; ctx->last_block = kThreads;
-  return ls.end();
+  return launch_timed(ctx, wait_stream, comm_stream, 11, select_k456(ctx->world, false), grid, kThreads, 0, P);
 }
 
 int b2d_sharded_step64(b2d_ctx* ctx, int slot, const float* grads, float* params, float* exp_avg,
@@ -1500,16 +1431,15 @@ int b2d_allgather(b2d_ctx* ctx, float* buf, size_t n, const int64_t* shard_off, 
 
 // ---- sharded path on the staged machinery (b2d_owner.cuh) ----------------------------------------------------
 int b2d_bucket_register(b2d_ctx* ctx, int bucket_id, const b2d_seg* segs, int nseg, int wire) {
-  int rc = check_ready(ctx);
-  if (rc != B2D_OK) return rc;
-  std::lock_guard<std::mutex> lk(ctx->mu);
+  Entry en(ctx, true);
+  if (en.rc != B2D_OK) return en.rc;
   if (segs == nullptr || nseg < 1) return fail(ctx, B2D_ERR_INVALID, "a reduce bucket needs at least one segment");
   if (wire != B2D_WIRE_FP32 && wire != B2D_WIRE_BF16) return fail(ctx, B2D_ERR_INVALID, "bad wire %d", wire);
   OwnerTable t;
   const std::string bad = build_owner_table(segs, nseg, ctx->world, wire, &t);
   if (!bad.empty()) return fail(ctx, B2D_ERR_INVALID, "%s", bad.c_str());
-  DeviceGuard guard(ctx->device);
-  rc = drop_bucket(ctx, ctx->owner_buckets, bucket_id);
+  int rc = en.use_device();
+  if (rc == B2D_OK) rc = drop_bucket(ctx, ctx->owner_buckets, bucket_id);
   if (rc != B2D_OK) return rc;
   b2d_ctx::OwnerBucket nb;
   nb.nseg = static_cast<int>(t.flat_off.size()); nb.wire = wire;
@@ -1523,9 +1453,8 @@ int b2d_bucket_register(b2d_ctx* ctx, int bucket_id, const b2d_seg* segs, int ns
 
 int b2d_reduce_to_owner(b2d_ctx* ctx, int bucket_id, float* grads, float* reduced, const int64_t* shard_off, float scale,
                         unsigned flags, unsigned phases, void* wait_stream, void* comm_stream) {
-  int rc = check_ready(ctx);
-  if (rc != B2D_OK) return rc;
-  std::lock_guard<std::mutex> lk(ctx->mu);
+  Entry en(ctx, true);
+  if (en.rc != B2D_OK) return en.rc;
   auto it = ctx->owner_buckets.find(bucket_id);
   if (it == ctx->owner_buckets.end()) return fail(ctx, B2D_ERR_STATE, "reduce bucket %d has not been registered", bucket_id);
   if (grads == nullptr || reduced == nullptr || shard_off == nullptr) return fail(ctx, B2D_ERR_INVALID, "NULL argument");
@@ -1533,9 +1462,8 @@ int b2d_reduce_to_owner(b2d_ctx* ctx, int bucket_id, float* grads, float* reduce
   const bool nvls = (flags & B2D_RTO_NVLS) != 0;
   if (nvls && !ctx->mc_bound) return fail(ctx, B2D_ERR_UNSUPPORTED, "NVLS requested but no multicast object is bound");
   b2d_ctx::OwnerBucket& ob = it->second;
-  DeviceGuard guard(ctx->device);
-  if (!guard.ok) return fail(ctx, B2D_ERR_CUDA, "cudaSetDevice(%d) failed", ctx->device);
-  rc = ensure_streams(ctx);
+  int rc = en.use_device();
+  if (rc == B2D_OK) rc = ensure_streams(ctx);
   if (rc != B2D_OK) return rc;
   cudaStream_t comm = static_cast<cudaStream_t>(comm_stream);
   const bool bf16 = ob.wire == B2D_WIRE_BF16;
@@ -1556,11 +1484,9 @@ int b2d_reduce_to_owner(b2d_ctx* ctx, int bucket_id, float* grads, float* reduce
   set_peer_wait(ctx, &P);
   cudaEvent_t es = nullptr;
   if (phases & 1u) {
-    rc = stream_wait(ctx, ctx->s_stage, static_cast<cudaStream_t>(wait_stream));
+    rc = join(ctx, ctx->s_stage, static_cast<cudaStream_t>(wait_stream));
     if (rc != B2D_OK) return rc;
-    const int grid = stream_grid(ctx, total);
-    if (bf16) seg_stage_kernel<true><<<grid, kStThreads, 0, ctx->s_stage>>>(P); else seg_stage_kernel<false><<<grid, kStThreads, 0, ctx->s_stage>>>(P);
-    ctx->launches += 1;
+    launch(ctx, select_seg_stage(bf16), stream_grid(ctx, total), kStThreads, 0, ctx->s_stage, P);
     es = next_event(ctx);
     B2D_CUDA(ctx, cudaEventRecord(es, ctx->s_stage));
   }
@@ -1569,21 +1495,16 @@ int b2d_reduce_to_owner(b2d_ctx* ctx, int bucket_id, float* grads, float* reduce
     const size_t mine = ob.owner_pack[ctx->rank + 1] - ob.owner_pack[ctx->rank];
     const size_t per_thread = nvls ? 8 : (kMaxLoadsInFlight / ctx->world > 1 ? kMaxLoadsInFlight / ctx->world : 1);
     const int grid = clamp_grid(mine, kExThreads * per_thread, ctx->exch_ctas);
-    TimingPair tp{nullptr, nullptr};
-    const bool timing = (ctx->flags & B2D_FLAG_TIMING) && take_timing_pair(ctx, &tp);
-    if (timing) B2D_CUDA(ctx, cudaEventRecord(tp.first, ctx->s_xfer));
-    if (bf16) { if (nvls) launch_seg_reduce<true, true>(P, ctx->world, grid, ctx->s_xfer); else launch_seg_reduce<true, false>(P, ctx->world, grid, ctx->s_xfer); }
-    else      { if (nvls) launch_seg_reduce<false, true>(P, ctx->world, grid, ctx->s_xfer); else launch_seg_reduce<false, false>(P, ctx->world, grid, ctx->s_xfer); }
-    ctx->launches += 1; ctx->exch_launches += 1;
-    if (timing) { B2D_CUDA(ctx, cudaEventRecord(tp.second, ctx->s_xfer)); ctx->exch_pending.push_back(tp); }
-    cudaEvent_t ex = next_event(ctx);
-    B2D_CUDA(ctx, cudaEventRecord(ex, ctx->s_xfer));
-    B2D_CUDA(ctx, cudaStreamWaitEvent(comm, ex, 0));
+    TimedSpan span(ctx, ctx->exch_pending);
+    if ((rc = span.start(ctx->s_xfer)) != B2D_OK) return rc;
+    launch(ctx, select_seg_reduce(ctx->world, bf16, nvls), grid, kExThreads, 0, ctx->s_xfer, P);
+    ctx->exch_launches += 1;
+    if ((rc = span.stop(ctx->s_xfer)) != B2D_OK || (rc = join(ctx, comm, ctx->s_xfer)) != B2D_OK) return rc;
     ctx->last_grid = grid;
     ob.op_epoch = 0;
   }
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return fail(ctx, B2D_ERR_CUDA, "kernel launch failed: %s", cudaGetErrorString(e));
+  rc = launch_result(ctx);
+  if (rc != B2D_OK) return rc;
   ctx->last_algo = 12; ctx->last_block = kExThreads;
   return B2D_OK;
 }
@@ -1592,16 +1513,15 @@ int b2d_reduce_to_owner(b2d_ctx* ctx, int bucket_id, float* grads, float* reduce
 static int adam_push(b2d_ctx* ctx, float* params, float* exp_avg, float* exp_avg_sq, const float* reduced, size_t n,
                      const int64_t* shard_off, const b2d_adam_group64* groups, int ngroups, unsigned flags, unsigned phases,
                      void* wait_stream, void* comm_stream, const float* grad_scale) {
-  int rc = check_ready(ctx);
-  if (rc != B2D_OK) return rc;
-  std::lock_guard<std::mutex> lk(ctx->mu);
+  Entry en(ctx, true);
+  if (en.rc != B2D_OK) return en.rc;
   if (params == nullptr || shard_off == nullptr) return fail(ctx, B2D_ERR_INVALID, "NULL argument");
   if (ngroups < 0 || ngroups > kMaxAdamGroups) return fail(ctx, B2D_ERR_INVALID, "at most %d parameter groups", kMaxAdamGroups);
   if (ngroups > 0 && (groups == nullptr || exp_avg == nullptr || exp_avg_sq == nullptr || reduced == nullptr))
     return fail(ctx, B2D_ERR_INVALID, "groups / exp_avg / exp_avg_sq / reduced are NULL");
   if ((phases & 6u) == 0 || (phases & ~6u) != 0) return fail(ctx, B2D_ERR_INVALID, "bad phase mask %u (bit 1 step + push, bit 2 wait)", phases);
   size_t max_len = 0;
-  rc = check_shard_off(ctx, shard_off, n, &max_len);
+  int rc = check_shard_off(ctx, shard_off, n, &max_len);
   if (rc != B2D_OK) return rc;
   const bool nvls = (flags & B2D_RTO_NVLS) != 0;
   if (nvls && !ctx->mc_bound) return fail(ctx, B2D_ERR_UNSUPPORTED, "NVLS requested but no multicast object is bound");
@@ -1609,9 +1529,8 @@ static int adam_push(b2d_ctx* ctx, float* params, float* exp_avg, float* exp_avg
   if (p8 < ctx->arena || p8 + n * 4 > ctx->arena + ctx->arena_bytes)
     return fail(ctx, B2D_ERR_INVALID, "the flat parameter buffer must live in the symmetric arena (b2d_arena_alloc)");
   if (n == 0) return B2D_OK;
-  DeviceGuard guard(ctx->device);
-  if (!guard.ok) return fail(ctx, B2D_ERR_CUDA, "cudaSetDevice(%d) failed", ctx->device);
-  rc = ensure_streams(ctx);
+  rc = en.use_device();
+  if (rc == B2D_OK) rc = ensure_streams(ctx);
   if (rc != B2D_OK) return rc;
   cudaStream_t comm = static_cast<cudaStream_t>(comm_stream);
   if (phases & 2u) ctx->push_epoch = ++ctx->epoch;
@@ -1631,41 +1550,30 @@ static int adam_push(b2d_ctx* ctx, float* params, float* exp_avg, float* exp_avg
     }
     P.rank = ctx->rank; P.world = ctx->world; P.epoch = ctx->push_epoch; P.peers = ctx->peers;
     P.grad_scale = grad_scale;
-    rc = stream_wait(ctx, ctx->s_xfer, static_cast<cudaStream_t>(wait_stream));
+    rc = join(ctx, ctx->s_xfer, static_cast<cudaStream_t>(wait_stream));
     if (rc != B2D_OK) return rc;
     // the step is not overlapped with anything and moves 28 B of local HBM traffic per owned element: one full wave
     // (3 CTAs of 256 threads x 68 registers per SM on sm_90a); a 128-CTA grid leaves most warp slots idle
     const int grid = clamp_grid(static_cast<size_t>(P.hi - P.lo) / 4, kExThreads * 2, static_cast<size_t>(ctx->sm_count) * 3);
-    TimingPair tp{nullptr, nullptr};
-    const bool timing = (ctx->flags & B2D_FLAG_TIMING) && take_timing_pair(ctx, &tp);
-    if (timing) B2D_CUDA(ctx, cudaEventRecord(tp.first, ctx->s_xfer));
-    dispatch_world(ctx->world, [&](auto w) {
-      constexpr int W = decltype(w)::value;
-      if (grad_scale != nullptr) {
-        if (nvls) adam_push_scaled_kernel<W, true><<<grid, kExThreads, 0, ctx->s_xfer>>>(P); else adam_push_scaled_kernel<W, false><<<grid, kExThreads, 0, ctx->s_xfer>>>(P);
-      } else {
-        if (nvls) adam_push_kernel<W, true><<<grid, kExThreads, 0, ctx->s_xfer>>>(P); else adam_push_kernel<W, false><<<grid, kExThreads, 0, ctx->s_xfer>>>(P);
-      }
-    });
-    ctx->launches += 1;
-    if (timing) { B2D_CUDA(ctx, cudaEventRecord(tp.second, ctx->s_xfer)); ctx->ev_pending.push_back(tp); }
+    TimedSpan span(ctx, ctx->ev_pending);
+    if ((rc = span.start(ctx->s_xfer)) != B2D_OK) return rc;
+    launch(ctx, select_adam_push(ctx->world, nvls, grad_scale != nullptr), grid, kExThreads, 0, ctx->s_xfer, P);
+    if ((rc = span.stop(ctx->s_xfer)) != B2D_OK) return rc;
     ctx->last_grid = grid;
   }
   if (phases & 4u) {
     ExParams XP{};
     XP.epoch = ctx->push_epoch;
     set_peer_wait(ctx, &XP);
-    cudaEvent_t ex = next_event(ctx);
-    B2D_CUDA(ctx, cudaEventRecord(ex, ctx->s_xfer));
-    B2D_CUDA(ctx, cudaStreamWaitEvent(ctx->s_unstage, ex, 0));
-    wait_published_kernel<<<1, 32, 0, ctx->s_unstage>>>(XP);
-    ctx->launches += 1;
+    rc = join(ctx, ctx->s_unstage, ctx->s_xfer);
+    if (rc != B2D_OK) return rc;
+    launch(ctx, wait_published_kernel, 1, 32, 0, ctx->s_unstage, XP);
     rc = join_unstage(ctx, comm);
     if (rc != B2D_OK) return rc;
     ctx->push_epoch = 0;
   }
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return fail(ctx, B2D_ERR_CUDA, "kernel launch failed: %s", cudaGetErrorString(e));
+  rc = launch_result(ctx);
+  if (rc != B2D_OK) return rc;
   ctx->last_algo = 13; ctx->last_block = kExThreads;
   return B2D_OK;
 }
@@ -1730,9 +1638,8 @@ int b2d_clip_register(b2d_ctx* ctx, size_t* offset) {
 
 int b2d_clip_norm(b2d_ctx* ctx, const float* x, size_t n, float max_norm, float* norm_out, float* coef_out, unsigned phases,
                   void* wait_stream, void* comm_stream) {
-  int rc = check_ready(ctx);
-  if (rc != B2D_OK) return rc;
-  std::lock_guard<std::mutex> lk(ctx->mu);
+  Entry en(ctx, true);
+  if (en.rc != B2D_OK) return en.rc;
   if (!ctx->clip_registered) return fail(ctx, B2D_ERR_STATE, "b2d_clip_norm before b2d_clip_register");
   if ((phases & 3u) == 0 || phases > 3u) return fail(ctx, B2D_ERR_INVALID, "bad phase mask %u (bit 0 partial, bit 1 coefficient)", phases);
   if (!(max_norm >= 0.f) || !isfinite(max_norm)) return fail(ctx, B2D_ERR_INVALID, "max_norm must be finite and >= 0 (got %g)", static_cast<double>(max_norm));
@@ -1740,14 +1647,13 @@ int b2d_clip_norm(b2d_ctx* ctx, const float* x, size_t n, float max_norm, float*
   if ((phases & 2u) && (norm_out == nullptr || coef_out == nullptr)) return fail(ctx, B2D_ERR_INVALID, "NULL output");
   if ((phases & 1u) && ctx->clip_op_epoch != 0) return fail(ctx, B2D_ERR_STATE, "clip partial issued again before the previous one was combined");
   if (!(phases & 1u) && ctx->clip_op_epoch == 0) return fail(ctx, B2D_ERR_STATE, "clip coefficient issued before the partial");
-  DeviceGuard guard(ctx->device);
-  if (!guard.ok) return fail(ctx, B2D_ERR_CUDA, "cudaSetDevice(%d) failed", ctx->device);
-  rc = ensure_streams(ctx);
+  int rc = en.use_device();
+  if (rc == B2D_OK) rc = ensure_streams(ctx);
   if (rc != B2D_OK) return rc;
   // on s_xfer, behind the reduce buckets (K12) that wrote the shard
   const size_t gen_bytes = static_cast<size_t>(ctx->world) * kClipSlotBytes;
   if (phases & 1u) {
-    rc = stream_wait(ctx, ctx->s_xfer, static_cast<cudaStream_t>(wait_stream));
+    rc = join(ctx, ctx->s_xfer, static_cast<cudaStream_t>(wait_stream));
     if (rc != B2D_OK) return rc;
     ctx->clip_gen = ctx->clip_calls++ & 1u;
     ctx->clip_op_epoch = ++ctx->clip_epoch;
@@ -1756,8 +1662,7 @@ int b2d_clip_norm(b2d_ctx* ctx, const float* x, size_t n, float max_norm, float*
     P.block_sums = reinterpret_cast<double*>(ctx->arena + ctx->clip_off + 2 * gen_bytes);
     P.region_off = ctx->clip_off + ctx->clip_gen * gen_bytes;
     P.rank = ctx->rank; P.world = ctx->world; P.epoch = ctx->clip_op_epoch; P.peers = ctx->peers;
-    sqnorm_partial_kernel<<<clip_grid(n, kClipGMax), kClipThreads, 0, ctx->s_xfer>>>(P);
-    ctx->launches += 1;
+    launch(ctx, sqnorm_partial_kernel, static_cast<int>(clip_grid(n, kClipGMax)), kClipThreads, 0, ctx->s_xfer, P);
   }
   if (phases & 2u) {
     ClipCoefParams P{};
@@ -1765,23 +1670,19 @@ int b2d_clip_norm(b2d_ctx* ctx, const float* x, size_t n, float max_norm, float*
     P.max_norm = max_norm; P.norm_out = norm_out; P.coef_out = coef_out;
     set_peer_wait(ctx, &P);
     P.epoch = ctx->clip_op_epoch;
-    clip_coef_kernel<<<1, 32, 0, ctx->s_xfer>>>(P);
-    ctx->launches += 1;
-    cudaEvent_t ex = next_event(ctx);
-    B2D_CUDA(ctx, cudaEventRecord(ex, ctx->s_xfer));
-    B2D_CUDA(ctx, cudaStreamWaitEvent(static_cast<cudaStream_t>(comm_stream), ex, 0));
+    launch(ctx, clip_coef_kernel, 1, 32, 0, ctx->s_xfer, P);
+    rc = join(ctx, static_cast<cudaStream_t>(comm_stream), ctx->s_xfer);
+    if (rc != B2D_OK) return rc;
     ctx->clip_op_epoch = 0;
   }
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return fail(ctx, B2D_ERR_CUDA, "kernel launch failed: %s", cudaGetErrorString(e));
-  return B2D_OK;
+  return launch_result(ctx);
 }
 
 // ---- optimizer in backward (f-2) ----------------------------------------------------------------------------------
 int b2d_optim_register(b2d_ctx* ctx, int bucket_id, float* const* params, float* const* state1, float* const* state2,
                        const int64_t* bucket_off, const int64_t* numel, int nparam) {
-  if (ctx == nullptr) return fail(nullptr, B2D_ERR_INVALID, "ctx is NULL");
-  std::lock_guard<std::mutex> lk(ctx->mu);
+  Entry en(ctx, false);
+  if (en.rc != B2D_OK) return en.rc;
   if (params == nullptr || bucket_off == nullptr || numel == nullptr || nparam < 1) return fail(ctx, B2D_ERR_INVALID, "bad parameter table");
   std::vector<float*> ptr(3 * static_cast<size_t>(nparam), nullptr);
   std::vector<unsigned> start(nparam + 1);
@@ -1796,8 +1697,8 @@ int b2d_optim_register(b2d_ctx* ctx, int bucket_id, float* const* params, float*
     if (cur > 0xffffffffll) return fail(ctx, B2D_ERR_INVALID, "bucket too large");
   }
   start[nparam] = static_cast<unsigned>(cur);
-  DeviceGuard guard(ctx->device);
-  int rc = drop_bucket(ctx, ctx->optim_buckets, bucket_id);
+  int rc = en.use_device();
+  if (rc == B2D_OK) rc = drop_bucket(ctx, ctx->optim_buckets, bucket_id);
   if (rc != B2D_OK) return rc;
   b2d_ctx::OptimBucket ob;
   ob.nseg = nparam; ob.n = static_cast<size_t>(cur);
@@ -1817,14 +1718,15 @@ int b2d_bucket_optim(b2d_ctx* ctx, int bucket_id, const float* grads, size_t n, 
 
 int b2d_bucket_optim64(b2d_ctx* ctx, int bucket_id, const float* grads, size_t n, int kind, const b2d_adam64* hp,
                        float momentum, void* stream) {
-  if (ctx == nullptr) return fail(nullptr, B2D_ERR_INVALID, "ctx is NULL");
-  std::lock_guard<std::mutex> lk(ctx->mu);
+  Entry en(ctx, false);
+  if (en.rc != B2D_OK) return en.rc;
   auto it = ctx->optim_buckets.find(bucket_id);
   if (it == ctx->optim_buckets.end()) return fail(ctx, B2D_ERR_STATE, "bucket %d has no parameter table (b2d_optim_register)", bucket_id);
   if (it->second.n != n) return fail(ctx, B2D_ERR_INVALID, "bucket %d has %zu elements, its parameter table covers %zu", bucket_id, n, it->second.n);
   if (grads == nullptr || hp == nullptr || (kind != 0 && kind != 1)) return fail(ctx, B2D_ERR_INVALID, "bad argument");
   if (kind == 1 && hp->step < 1) return fail(ctx, B2D_ERR_INVALID, "Adam needs step >= 1");
-  DeviceGuard guard(ctx->device);
+  const int rc = en.use_device();
+  if (rc != B2D_OK) return rc;
   OptimParams P{};
   P.param_ptr = it->second.d_ptr; P.seg_start = it->second.d_start; P.nseg = it->second.nseg;
   P.state1_ptr = it->second.d_ptr + it->second.nseg; P.state2_ptr = it->second.d_ptr + 2 * it->second.nseg;
@@ -1833,20 +1735,16 @@ int b2d_bucket_optim64(b2d_ctx* ctx, int bucket_id, const float* grads, size_t n
   P.first_step = hp->step <= 1;
   if (kind == 1) P.adam = adam_consts(*hp);
   const int grid = clamp_grid(n, kStThreads * 4, static_cast<size_t>(ctx->sm_count) * 2);
-  bucket_optim_kernel<<<grid, kStThreads, 0, static_cast<cudaStream_t>(stream)>>>(P);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return fail(ctx, B2D_ERR_CUDA, "kernel launch failed: %s", cudaGetErrorString(e));
-  ctx->launches += 1;
-  return B2D_OK;
+  launch(ctx, bucket_optim_kernel, grid, kStThreads, 0, static_cast<cudaStream_t>(stream), P);
+  return launch_result(ctx);
 }
 
 int b2d_barrier(b2d_ctx* ctx, void* stream) {
-  int rc = check_ready(ctx);
-  if (rc != B2D_OK) return rc;
-  std::lock_guard<std::mutex> lk(ctx->mu);
+  Entry en(ctx, true);
+  if (en.rc != B2D_OK) return en.rc;
   if (ctx->world == 1) return B2D_OK;
-  DeviceGuard guard(ctx->device);
-  return launch_barrier(ctx, static_cast<cudaStream_t>(stream));
+  const int rc = en.use_device();
+  return rc != B2D_OK ? rc : launch_barrier(ctx, static_cast<cudaStream_t>(stream));
 }
 
 // ---- synchronised BatchNorm (b2d_syncbn.cuh) -----------------------------------------------
@@ -1878,9 +1776,8 @@ int b2d_bn_register(b2d_ctx* ctx, int layer_id, int channels, size_t* offset) {
 static int bn_exchange(b2d_ctx* ctx, int layer_id, bool fwd, const float* a, const float* b, float count, float eps,
                        float momentum, float* out_a, float* out_b, int32_t* counts, float* running_mean, float* running_var,
                        unsigned phases, void* stream) {
-  int rc = check_ready(ctx);
-  if (rc != B2D_OK) return rc;
-  std::lock_guard<std::mutex> lk(ctx->mu);
+  Entry en(ctx, true);
+  if (en.rc != B2D_OK) return en.rc;
   auto it = ctx->bn_layers.find(layer_id);
   if (it == ctx->bn_layers.end()) return fail(ctx, B2D_ERR_STATE, "BatchNorm layer %d has not been registered", layer_id);
   if ((phases & 3u) == 0 || phases > 3u) return fail(ctx, B2D_ERR_INVALID, "bad phase mask %u (bit 0 push, bit 1 combine)", phases);
@@ -1895,8 +1792,8 @@ static int bn_exchange(b2d_ctx* ctx, int layer_id, bool fwd, const float* a, con
     return fail(ctx, B2D_ERR_STATE, "BatchNorm layer %d: push issued again before the previous exchange was combined", layer_id);
   if (!(phases & 1u) && L.op_epoch[d] == 0)
     return fail(ctx, B2D_ERR_STATE, "BatchNorm layer %d: combine issued before the push", layer_id);
-  DeviceGuard guard(ctx->device);
-  if (!guard.ok) return fail(ctx, B2D_ERR_CUDA, "cudaSetDevice(%d) failed", ctx->device);
+  const int rc = en.use_device();
+  if (rc != B2D_OK) return rc;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int C = L.channels;
   const size_t W = static_cast<size_t>(ctx->world);
@@ -1909,8 +1806,7 @@ static int bn_exchange(b2d_ctx* ctx, int layer_id, bool fwd, const float* a, con
     P.a = a; P.b = b; P.count = fwd ? count : 0.f; P.channels = C; P.fwd = fwd ? 1 : 0;
     P.region_off = base + L.op_gen[d] * gen_bytes;
     P.rank = ctx->rank; P.world = ctx->world; P.epoch = L.op_epoch[d]; P.peers = ctx->peers;
-    bn_push_kernel<<<1, kBnThreads, 0, st>>>(P);
-    ctx->launches += 1;
+    launch(ctx, bn_push_kernel, 1, kBnThreads, 0, st, P);
   }
   if (phases & 2u) {
     BnCombineParams P{};
@@ -1921,13 +1817,10 @@ static int bn_exchange(b2d_ctx* ctx, int layer_id, bool fwd, const float* a, con
     set_peer_wait(ctx, &P);
     P.epoch = L.op_epoch[d];
     const int grid = clamp_grid(static_cast<size_t>(C), kBnThreads, static_cast<size_t>(ctx->sm_count));
-    if (fwd) bn_combine_kernel<true><<<grid, kBnThreads, 0, st>>>(P); else bn_combine_kernel<false><<<grid, kBnThreads, 0, st>>>(P);
-    ctx->launches += 1;
+    launch(ctx, select_bn_combine(fwd), grid, kBnThreads, 0, st, P);
     L.op_epoch[d] = 0;
   }
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return fail(ctx, B2D_ERR_CUDA, "kernel launch failed: %s", cudaGetErrorString(e));
-  return B2D_OK;
+  return launch_result(ctx);
 }
 
 int b2d_bn_stats_exchange(b2d_ctx* ctx, int layer_id, const float* mean, const float* invstd, float count, float eps,
@@ -1972,12 +1865,12 @@ int b2d_arena_reset(b2d_ctx* ctx) {
 
 // ---- link probe ----------------------------------------------------------------------------
 int b2d_peer_bw(b2d_ctx* ctx, int peer, size_t bytes, int iters, int mode, double* gbps) {
-  int rc = check_ready(ctx);
-  if (rc != B2D_OK) return rc;
+  Entry en(ctx, true);
+  if (en.rc != B2D_OK) return en.rc;
   if (gbps == nullptr || peer < 0 || peer >= ctx->world) return fail(ctx, B2D_ERR_INVALID, "bad peer/gbps");
   if (iters < 1) iters = 1;
-  std::lock_guard<std::mutex> lk(ctx->mu);
-  DeviceGuard guard(ctx->device);
+  const int rc = en.use_device();
+  if (rc != B2D_OK) return rc;
   bytes = bytes / 16 * 16;
   if (bytes == 0 || kSignalBytes + bytes > ctx->arena_bytes) return fail(ctx, B2D_ERR_INVALID, "probe size must fit the arena");
   void* dst = nullptr;

@@ -1,7 +1,8 @@
 // b2d_launch.cuh — the host-side decisions around the kernel launches that b2d.cu and the CPU emulator
-// (emu/emu_harness.cpp) share: which specialisation of a kernel a world size runs, Adam's host constants, the chunk
-// geometry of the staged exchange and the owner-segment table of a reduce bucket.  Pure host code without CUDA
-// runtime calls, so that the emulated launches exercise the very decisions the library makes.
+// (emu/emu_harness.cpp) share: which template specialisation of a kernel family the runtime choices select, the
+// peer-wait fields of a kernel's parameters, Adam's host constants, the chunk geometry of the staged exchange and the
+// owner-segment table of a reduce bucket.  Pure host code without CUDA runtime calls, so that the emulated launches
+// exercise the very decisions the library makes.
 #pragma once
 
 #include <math.h>
@@ -12,19 +13,95 @@
 #include <vector>
 
 #include "b2d_kernels.cuh"
+#include "b2d_owner.cuh"
+#include "b2d_staged.cuh"
+#include "b2d_syncbn.cuh"
 
 namespace b2d {
 
 // The kernels that read peers are specialised for 2, 4 and 8 ranks; W = 0 is the generic build for any other world
-// size.  Calls f(std::integral_constant<int, W>{}) with the specialisation that `world` runs.
+// size.  Returns f(std::integral_constant<int, W>{}) for the specialisation that `world` runs.
 template <typename F>
-void dispatch_world(int world, F&& f) {
+auto dispatch_world(int world, F&& f) {
   switch (world) {
-    case 2: f(std::integral_constant<int, 2>{}); break;
-    case 4: f(std::integral_constant<int, 4>{}); break;
-    case 8: f(std::integral_constant<int, 8>{}); break;
-    default: f(std::integral_constant<int, 0>{}); break;
+    case 2: return f(std::integral_constant<int, 2>{});
+    case 4: return f(std::integral_constant<int, 4>{});
+    case 8: return f(std::integral_constant<int, 8>{});
+    default: return f(std::integral_constant<int, 0>{});
   }
+}
+
+// ---- kernel selectors ----------------------------------------------------------------------------------------------
+// One per templated kernel family: the runtime choices in, the kernel to launch out.  The library launches
+// select_...(...)<<<grid, block, smem, stream>>>(P), the emulator calls the returned function, and b2d.cu's
+// preload_kernels walks every selector over its whole domain, so any kernel a selector can return is loaded up front.
+// (K2T's selector lives in b2d.cu: the emulator does not compile b2d_tma.cuh.)
+inline auto select_k0(bool bf16) { return bf16 ? &k0_cast_scale_kernel<true> : &k0_cast_scale_kernel<false>; }
+
+inline auto select_k1(int world, bool bf16) {
+  return dispatch_world(world, [=](auto w) {
+    constexpr int W = decltype(w)::value;
+    return bf16 ? &k1_one_shot_kernel<W, true> : &k1_one_shot_kernel<W, false>;
+  });
+}
+
+inline auto select_k2(int world, bool bf16, bool nvls_fused) {
+  return dispatch_world(world, [=](auto w) {
+    constexpr int W = decltype(w)::value;
+    if (bf16) return nvls_fused ? &k2_two_shot_kernel<W, true, true> : &k2_two_shot_kernel<W, true, false>;
+    return nvls_fused ? &k2_two_shot_kernel<W, false, true> : &k2_two_shot_kernel<W, false, false>;
+  });
+}
+
+inline auto select_k456(int world, bool bf16) {
+  return dispatch_world(world, [=](auto w) {
+    constexpr int W = decltype(w)::value;
+    return bf16 ? &k456_sharded_kernel<W, true> : &k456_sharded_kernel<W, false>;
+  });
+}
+
+inline auto select_stage(bool bf16) { return bf16 ? &stage_kernel<true> : &stage_kernel<false>; }
+inline auto select_unstage(bool bf16) { return bf16 ? &unstage_kernel<true> : &unstage_kernel<false>; }
+
+// An in-place exchange reads the fp32 bucket itself, so `inplace` ignores `bf16`: there is no bf16 in-place kernel.
+inline auto select_exch(int world, bool bf16, bool nvls, bool inplace) {
+  return dispatch_world(world, [=](auto w) {
+    constexpr int W = decltype(w)::value;
+    if (inplace) return nvls ? &exch_kernel<W, false, true, true> : &exch_kernel<W, false, false, true>;
+    if (bf16) return nvls ? &exch_kernel<W, true, true, false> : &exch_kernel<W, true, false, false>;
+    return nvls ? &exch_kernel<W, false, true, false> : &exch_kernel<W, false, false, false>;
+  });
+}
+
+inline auto select_seg_stage(bool bf16) { return bf16 ? &seg_stage_kernel<true> : &seg_stage_kernel<false>; }
+
+inline auto select_seg_reduce(int world, bool bf16, bool nvls) {
+  return dispatch_world(world, [=](auto w) {
+    constexpr int W = decltype(w)::value;
+    if (bf16) return nvls ? &seg_reduce_kernel<W, true, true> : &seg_reduce_kernel<W, true, false>;
+    return nvls ? &seg_reduce_kernel<W, false, true> : &seg_reduce_kernel<W, false, false>;
+  });
+}
+
+// scaled: K13 with the gradients multiplied by *grad_scale on the device (adam_push_scaled_kernel)
+inline auto select_adam_push(int world, bool nvls, bool scaled) {
+  return dispatch_world(world, [=](auto w) {
+    constexpr int W = decltype(w)::value;
+    if (scaled) return nvls ? &adam_push_scaled_kernel<W, true> : &adam_push_scaled_kernel<W, false>;
+    return nvls ? &adam_push_kernel<W, true> : &adam_push_kernel<W, false>;
+  });
+}
+
+inline auto select_bn_combine(bool fwd) { return fwd ? &bn_combine_kernel<true> : &bn_combine_kernel<false>; }
+
+// The fields of a kernel's parameters that let it wait for peers: who is who, and the watchdog (0: never trap).
+template <typename Params>
+void set_peer_wait(Params* P, int rank, int world, const Peers& peers, unsigned long long timeout_ns, Diag* diag) {
+  P->rank = rank;
+  P->world = world;
+  P->peers = peers;
+  P->timeout_ns = timeout_ns;
+  P->diag = diag;
 }
 
 // Most blocks the global-norm kernel K18 (b2d_clip.cuh) runs: its summation order depends on this value and on the

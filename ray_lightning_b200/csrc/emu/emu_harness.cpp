@@ -1,4 +1,5 @@
-// emu_harness.cpp — runs the libb2d kernels (the very sources nvcc compiles) on CPU threads.
+// emu_harness.cpp — runs the libb2d kernels (the very sources nvcc compiles) on CPU threads, chosen by the same
+// selectors (b2d_launch.cuh) the library launches through.
 // TEST INFRASTRUCTURE ONLY: built by tests/test_kernel_emulation.py with g++ -std=c++20 -DB2D_EMU -pthread.
 // See emu/cuda_emu.h for what is and is not modelled.
 #ifndef B2D_EMU
@@ -80,28 +81,58 @@ Peers make_peers(const Group& g) {
   return p;
 }
 
-template <int W, bool BF16>
-void run_ar(int algo, const ArParams& P, int pipe_k) {
-  (void)pipe_k;
-  switch (algo) {
-    case 1: k1_one_shot_kernel<W, BF16>(P); break;
-    case 2: k2_two_shot_kernel<W, BF16, false>(P); break;
-    case 3: k2_two_shot_kernel<W, BF16, true>(P); break;
-    default: break;
-  }
-}
-
-// one kernel of one rank: grid x block threads, joined before returning (a stream runs these one after another)
-int launch_one(int grid, int block, std::function<void()> body) {
-  std::vector<std::function<void()>> bodies(1, std::move(body));
+// one kernel of one rank: grid x block threads running kernel(args...), joined before returning (a stream runs these
+// one after another)
+template <typename Kernel, typename... Args>
+int launch_one(Kernel kernel, int grid, int block, const Args&... args) {
+  std::vector<std::function<void()>> bodies(1, [=] { kernel(args...); });
   return launch_all(1, grid, block, bodies);
 }
 
-template <int W>
-void run_exch(const ExParams& P, bool bf16, bool nvls, bool inplace) {
-  if (inplace) { if (nvls) exch_kernel<W, false, true, true>(P); else exch_kernel<W, false, false, true>(P); }
-  else if (bf16) { if (nvls) exch_kernel<W, true, true, false>(P); else exch_kernel<W, true, false, false>(P); }
-  else { if (nvls) exch_kernel<W, false, true, false>(P); else exch_kernel<W, false, false, false>(P); }
+// The peer-wait fields of rank r's parameters, as b2d.cu fills them from its context (no diagnostics record here).
+template <typename Params>
+void set_peer_wait(Params* P, int r, const Group& g, unsigned long long timeout_s) {
+  set_peer_wait(P, r, g.world, make_peers(g), timeout_s * 1000000000ull, nullptr);
+}
+
+// Points the emulated multicast alias (NVLS) at the group's arenas.
+void bind_multicast(const Group& g) {
+  emu::Multicast& mc = emu::multicast();
+  mc.fake_base = g.fake_mc; mc.world = g.world;
+  for (int r = 0; r < g.world; ++r) mc.arena[r] = g.arena[r];
+}
+
+// Runs the phases of one operation, f(rank, chunk) for every rank and chunk of each phase.  `order`:
+//   0  every rank is one in-order stream (every phase of chunk 0, then of chunk 1, ...); the ranks run concurrently
+//   1  fully serialised, phase-major (the first phase of every chunk and rank, then the second, ...): what a
+//      serialising profiler makes of the single-GPU loopback ranks
+//   2  one concurrent stream per phase and rank, coupled ONLY by the kernels' flags — more freedom than the
+//      event-ordered streams of b2d.cu allow
+using Phase = std::function<int(int rank, int chunk)>;
+int run_phases(int world, int nchunks, int order, const std::vector<Phase>& phases) {
+  if (order == 1) {
+    for (const Phase& f : phases)
+      for (int c = 0; c < nchunks; ++c)
+        for (int r = 0; r < world; ++r)
+          if (f(r, c) != 0) return -1;
+    return 0;
+  }
+  std::atomic<int> bad{0};
+  std::vector<std::thread> streams;
+  for (int r = 0; r < world; ++r) {
+    if (order == 0) {
+      streams.emplace_back([&, r] {
+        for (int c = 0; c < nchunks; ++c)
+          for (const Phase& f : phases)
+            if (f(r, c) != 0) { bad = 1; break; }
+      });
+    } else {
+      for (const Phase& f : phases)
+        streams.emplace_back([&, r, fp = &f] { for (int c = 0; c < nchunks; ++c) if ((*fp)(r, c) != 0) bad = 1; });
+    }
+  }
+  for (auto& t : streams) t.join();
+  return bad.load() ? -1 : 0;
 }
 
 }  // namespace
@@ -132,12 +163,8 @@ size_t emu_signal_bytes(void) { return kSignalBytes; }
 
 // The staged exchange (b2d_staged.cuh) of one bucket, cut into chunks of `chunk_packs`, epochs epoch0.. (monotone
 // over calls, like ctx->epoch in b2d.cu).  wire_off: byte offset of the staging region in every arena; with
-// `inplace` the fp32 buckets themselves live there (bufs is ignored).  `order`:
-//   0  every rank is one in-order stream S,X,W,U per chunk; the ranks run concurrently
-//   1  fully serialised, phase-major (S of every rank, then X of every rank, then W+U): what a serialising
-//      profiler makes of the single-GPU loopback ranks
-//   2  three concurrent streams per rank (all S | all X | all W+U), coupled ONLY by the staged / published
-//      flags — more freedom than the event-ordered streams of b2d.cu allow
+// `inplace` the fp32 buckets themselves live there (bufs is ignored).  `order` as in run_phases, over the phases S,
+// X and W+U: 0 is b2d.cu's stream order, 1 and 2 are the serialised and the freest schedules.
 int emu_staged_allreduce(void* h, int nvls, int bf16, int inplace, float** bufs, size_t n, float scale, size_t wire_off,
                          size_t chunk_packs, int st_grid, int ex_grid, unsigned epoch0, int order, int use_generic_w) {
   Group* g = static_cast<Group*>(h);
@@ -146,116 +173,66 @@ int emu_staged_allreduce(void* h, int nvls, int bf16, int inplace, float** bufs,
   const size_t npacks = (n + epp - 1) / epp;
   if (wire_off + npacks * 16 > g->arena_bytes) return -4;
   const int nchunks = static_cast<int>((npacks + chunk_packs - 1) / chunk_packs);
-  emu::Multicast& mc = emu::multicast();
-  mc.fake_base = g->fake_mc; mc.world = world;
-  for (int r = 0; r < world; ++r) mc.arena[r] = g->arena[r];
-  const Peers peers = make_peers(*g);
-  auto S = [&](int r, int c) {
+  bind_multicast(*g);
+  auto stage_params = [&](int r, int c) {   // S and U of chunk c
     StParams P{};
-    P.scale = scale; P.rank = r; P.world = world; P.peers = peers;
-    if (inplace) {
-      if (c != 0) return 0;
-      P.epoch = epoch0 + nchunks - 1;
-      return launch_one(1, 32, [P] { arrive_kernel(P); });
-    }
+    P.scale = scale; P.rank = r; P.world = world; P.peers = make_peers(*g);
     const ChunkSpan cs = chunk_span(c, npacks, chunk_packs, n, epp);
     P.grad = bufs[r] + cs.p0 * epp;
     P.n = cs.n;
     P.wire = reinterpret_cast<uint4*>(g->arena[r] + wire_off) + cs.p0;
     P.epoch = epoch0 + c;
-    return bf16 ? launch_one(st_grid, kStThreads, [P] { stage_kernel<true>(P); }) : launch_one(st_grid, kStThreads, [P] { stage_kernel<false>(P); });
+    return P;
+  };
+  auto S = [&](int r, int c) {
+    if (!inplace) return launch_one(select_stage(bf16), st_grid, kStThreads, stage_params(r, c));
+    if (c != 0) return 0;
+    StParams P{};
+    P.rank = r; P.world = world; P.peers = make_peers(*g);
+    P.epoch = epoch0 + nchunks - 1;
+    return launch_one(arrive_kernel, 1, 32, P);
   };
   auto X = [&](int r, int c) {
     ExParams P{};
-    P.scale = scale; P.rank = r; P.world = world; P.peers = peers; P.timeout_ns = 120ull * 1000000000ull; P.diag = nullptr;
+    set_peer_wait(&P, r, *g, 120);
+    P.scale = scale;
     const ChunkSpan cs = chunk_span(c, npacks, chunk_packs, n, epp);
     P.wire_off = wire_off + cs.p0 * 16; P.npacks = cs.packs; P.epoch = epoch0 + c;
     P.n_valid = inplace ? cs.n_valid : 0;
-    return launch_one(ex_grid, kExThreads, [=] {
-      dispatch_world(use_generic_w ? 0 : world, [&](auto w) { run_exch<decltype(w)::value>(P, bf16 != 0, nvls != 0, inplace != 0); });
-    });
+    return launch_one(select_exch(use_generic_w ? 0 : world, bf16, nvls, inplace), ex_grid, kExThreads, P);
   };
   auto WU = [&](int r, int c) {
     ExParams P{};
-    P.rank = r; P.world = world; P.peers = peers; P.timeout_ns = 120ull * 1000000000ull; P.epoch = epoch0 + c;
-    int rc = launch_one(1, 32, [P] { wait_published_kernel(P); });
+    set_peer_wait(&P, r, *g, 120);
+    P.epoch = epoch0 + c;
+    const int rc = launch_one(wait_published_kernel, 1, 32, P);
     if (rc != 0 || inplace) return rc;
-    StParams Q{};
-    Q.scale = scale; Q.rank = r; Q.world = world; Q.peers = peers;
-    const ChunkSpan cs = chunk_span(c, npacks, chunk_packs, n, epp);
-    Q.grad = bufs[r] + cs.p0 * epp;
-    Q.n = cs.n;
-    Q.wire = reinterpret_cast<uint4*>(g->arena[r] + wire_off) + cs.p0;
-    Q.epoch = epoch0 + c;
-    return bf16 ? launch_one(st_grid, kStThreads, [Q] { unstage_kernel<true>(Q); }) : launch_one(st_grid, kStThreads, [Q] { unstage_kernel<false>(Q); });
+    return launch_one(select_unstage(bf16), st_grid, kStThreads, stage_params(r, c));
   };
-  std::atomic<int> bad{0};
-  if (order == 1) {
-    for (int c = 0; c < nchunks; ++c) for (int r = 0; r < world; ++r) if (S(r, c) != 0) return -1;
-    for (int c = 0; c < nchunks; ++c) for (int r = 0; r < world; ++r) if (X(r, c) != 0) return -1;
-    for (int c = 0; c < nchunks; ++c) for (int r = 0; r < world; ++r) if (WU(r, c) != 0) return -1;
-    return 0;
-  }
-  std::vector<std::thread> streams;
-  for (int r = 0; r < world; ++r) {
-    if (order == 0) {
-      streams.emplace_back([&, r] { for (int c = 0; c < nchunks; ++c) if (S(r, c) != 0 || X(r, c) != 0 || WU(r, c) != 0) bad = 1; });
-    } else {
-      streams.emplace_back([&, r] { for (int c = 0; c < nchunks; ++c) if (S(r, c) != 0) bad = 1; });
-      streams.emplace_back([&, r] { for (int c = 0; c < nchunks; ++c) if (X(r, c) != 0) bad = 1; });
-      streams.emplace_back([&, r] { for (int c = 0; c < nchunks; ++c) if (WU(r, c) != 0) bad = 1; });
-    }
-  }
-  for (auto& t : streams) t.join();
-  return bad.load() ? -1 : 0;
+  return run_phases(world, nchunks, order, {S, X, WU});
 }
 
 // K11 + K12 (b2d_owner.cuh): one reduce bucket given as an owner-sorted segment table (seg_start in packs of the wire
-// format, cumulative, nseg + 1 entries; owner_pack[world + 1]).  order as in emu_staged_allreduce (0 / 1).
+// format, cumulative, nseg + 1 entries; owner_pack[world + 1]).  order as in run_phases (0 / 1).
 int emu_reduce_to_owner(void* h, int bf16, int nvls, float** grads, float** reduced, const long long* shard_off,
                         const long long* seg_flat_off, const unsigned* seg_start, int nseg, const unsigned* owner_pack,
                         size_t wire_off, float scale, int zero_grads, int accumulate, unsigned epoch, int order, int use_generic_w) {
   Group* g = static_cast<Group*>(h);
   const int world = g->world;
   if (wire_off + static_cast<size_t>(seg_start[nseg]) * 16 > g->arena_bytes) return -4;
-  emu::Multicast& mc = emu::multicast();
-  mc.fake_base = g->fake_mc; mc.world = world;
-  for (int r = 0; r < world; ++r) mc.arena[r] = g->arena[r];
-  const Peers peers = make_peers(*g);
+  bind_multicast(*g);
   auto mk = [&](int r) {
     SegParams P{};
     P.seg_flat_off = seg_flat_off; P.seg_start = seg_start; P.nseg = nseg;
     for (int i = 0; i <= B2D_MAX_WORLD; ++i) P.owner_pack[i] = owner_pack[i <= world ? i : world];
     P.grads = grads[r]; P.reduced = reduced[r]; P.shard_lo = shard_off[r]; P.wire_off = wire_off; P.scale = scale;
-    P.zero_grads = zero_grads; P.accumulate = accumulate; P.rank = r; P.world = world; P.epoch = epoch;
-    P.timeout_ns = 120ull * 1000000000ull; P.diag = nullptr; P.peers = peers;
+    P.zero_grads = zero_grads; P.accumulate = accumulate; P.epoch = epoch;
+    set_peer_wait(&P, r, *g, 120);
     return P;
   };
-  auto S = [&](int r) {
-    const SegParams P = mk(r);
-    return bf16 ? launch_one(2, kStThreads, [P] { seg_stage_kernel<true>(P); }) : launch_one(2, kStThreads, [P] { seg_stage_kernel<false>(P); });
-  };
-  auto X = [&](int r) {
-    const SegParams P = mk(r);
-    auto run = [=] {
-      dispatch_world(use_generic_w ? 0 : world, [&](auto w) {
-        constexpr int W = decltype(w)::value;
-        if (bf16) { if (nvls) seg_reduce_kernel<W, true, true>(P); else seg_reduce_kernel<W, true, false>(P); }
-        else { if (nvls) seg_reduce_kernel<W, false, true>(P); else seg_reduce_kernel<W, false, false>(P); }
-      });
-    };
-    return launch_one(2, kExThreads, run);
-  };
-  if (order == 1) {
-    for (int r = 0; r < world; ++r) if (S(r) != 0) return -1;
-    for (int r = 0; r < world; ++r) if (X(r) != 0) return -1;
-    return 0;
-  }
-  std::atomic<int> bad{0};
-  std::vector<std::thread> streams;
-  for (int r = 0; r < world; ++r) streams.emplace_back([&, r] { if (S(r) != 0 || X(r) != 0) bad = 1; });
-  for (auto& t : streams) t.join();
-  return bad.load() ? -1 : 0;
+  auto S = [&](int r, int) { return launch_one(select_seg_stage(bf16), 2, kStThreads, mk(r)); };
+  auto X = [&](int r, int) { return launch_one(select_seg_reduce(use_generic_w ? 0 : world, bf16, nvls), 2, kExThreads, mk(r)); };
+  return run_phases(world, 1, order, {S, X});
 }
 
 // K13: params live in every arena at param_off; m, v, reduced are the ranks' own-shard buffers.  One Adam group per
@@ -267,11 +244,8 @@ static int adam_push_impl(void* h, int nvls, size_t param_off, float** m, float*
   Group* g = static_cast<Group*>(h);
   const int world = g->world;
   if (param_off + n * 4 > g->arena_bytes) return -4;
-  emu::Multicast& mc = emu::multicast();
-  mc.fake_base = g->fake_mc; mc.world = world;
-  for (int r = 0; r < world; ++r) mc.arena[r] = g->arena[r];
-  const Peers peers = make_peers(*g);
-  auto X = [&](int r) {
+  bind_multicast(*g);
+  auto X = [&](int r, int) {
     PushParams P{};
     P.params = reinterpret_cast<float*>(g->arena[r] + param_off); P.param_off = param_off;
     P.exp_avg = m ? m[r] : nullptr; P.exp_avg_sq = v ? v[r] : nullptr; P.reduced = reduced ? reduced[r] : nullptr;
@@ -280,32 +254,17 @@ static int adam_push_impl(void* h, int nvls, size_t param_off, float** m, float*
       P.group_lo[0] = glo[r]; P.group_hi[0] = ghi[r];
       P.group[0] = adam_consts(b2d_adam64{lr, beta1, beta2, eps, wd, step, adamw, 0, 0});
     }
-    P.rank = r; P.world = world; P.epoch = epoch; P.peers = peers;
+    P.rank = r; P.world = world; P.epoch = epoch; P.peers = make_peers(*g);
     P.grad_scale = grad_scale ? grad_scale[r] : nullptr;
-    auto run = [=] {
-      dispatch_world(use_generic_w ? 0 : world, [&](auto w) {
-        constexpr int W = decltype(w)::value;
-        if (P.grad_scale != nullptr) { if (nvls) adam_push_scaled_kernel<W, true>(P); else adam_push_scaled_kernel<W, false>(P); }
-        else { if (nvls) adam_push_kernel<W, true>(P); else adam_push_kernel<W, false>(P); }
-      });
-    };
-    return launch_one(2, kExThreads, run);
+    return launch_one(select_adam_push(use_generic_w ? 0 : world, nvls, grad_scale != nullptr), 2, kExThreads, P);
   };
-  auto Wt = [&](int r) {
+  auto Wt = [&](int r, int) {
     ExParams P{};
-    P.rank = r; P.world = world; P.peers = peers; P.timeout_ns = 120ull * 1000000000ull; P.epoch = epoch;
-    return launch_one(1, 32, [P] { wait_published_kernel(P); });
+    set_peer_wait(&P, r, *g, 120);
+    P.epoch = epoch;
+    return launch_one(wait_published_kernel, 1, 32, P);
   };
-  if (order == 1) {
-    for (int r = 0; r < world; ++r) if (X(r) != 0) return -1;
-    for (int r = 0; r < world; ++r) if (Wt(r) != 0) return -1;
-    return 0;
-  }
-  std::atomic<int> bad{0};
-  std::vector<std::thread> streams;
-  for (int r = 0; r < world; ++r) streams.emplace_back([&, r] { if (X(r) != 0 || Wt(r) != 0) bad = 1; });
-  for (auto& t : streams) t.join();
-  return bad.load() ? -1 : 0;
+  return run_phases(world, 1, order, {X, Wt});
 }
 
 // The *64 entry points take the hyper-parameters as doubles (b2d_adam64); the others as fp32 (b2d_adam), widened.
@@ -350,7 +309,7 @@ int emu_bucket_optim64(float** params, float** state1, float** state2, const uns
   P.grads = grads; P.n = n; P.kind = kind; P.lr = static_cast<float>(lr); P.momentum = momentum;
   P.weight_decay = static_cast<float>(wd); P.first_step = step <= 1;
   if (kind == 1) P.adam = adam_consts(b2d_adam64{lr, beta1, beta2, eps, wd, step, adamw, 0, 0});
-  return launch_one(2, kStThreads, [P] { bucket_optim_kernel(P); });
+  return launch_one(bucket_optim_kernel, 2, kStThreads, P);
 }
 
 int emu_bucket_optim(float** params, float** state1, float** state2, const unsigned* seg_start, int nseg, const float* grads,
@@ -368,32 +327,24 @@ int emu_allreduce(void* h, int algo, int bf16, float** bufs, size_t n, float sca
   const size_t npacks = (n + epp - 1) / epp, slice = (npacks + world - 1) / world;
   const size_t half = (slice * world * 16 + 255) / 256 * 256;
   if (kSignalBytes + 2 * half > g->arena_bytes) return -4;
-  emu::Multicast& mc = emu::multicast();
-  mc.fake_base = g->fake_mc; mc.world = world;
-  for (int r = 0; r < world; ++r) mc.arena[r] = g->arena[r];
-  std::vector<ArParams> params(world);
+  if (algo < 1 || algo > 3) return -2;
+  (void)pipe_k;
+  bind_multicast(*g);
+  const int w = use_generic_w ? 0 : world;
+  const auto kernel = algo == 1 ? select_k1(w, bf16) : select_k2(w, bf16, algo == 3);
   std::vector<std::function<void()>> bodies(world);
   for (int r = 0; r < world; ++r) {
     ArParams P{};
     P.trace = nullptr; P.grad = bufs[r]; P.n = n; P.stage_off = kSignalBytes + (parity & 1) * half; P.scale = scale;
-    P.rank = r; P.world = world; P.timeout_ns = 60ull * 1000000000ull; P.diag = nullptr; P.peers = make_peers(*g);
-    params[r] = P;
-    const ArParams* pp = &params[r];
-    dispatch_world(use_generic_w ? 0 : world, [&](auto w) {
-      constexpr int W = decltype(w)::value;
-      bodies[r] = bf16 ? std::function<void()>([=] { run_ar<W, true>(algo, *pp, pipe_k); })
-                       : std::function<void()>([=] { run_ar<W, false>(algo, *pp, pipe_k); });
-    });
+    set_peer_wait(&P, r, *g, 60);
+    bodies[r] = [=] { kernel(P); };
   }
   return launch_all(world, grid, kThreads, bodies);
 }
 
 // K0: world 1, no peers
 int emu_k0(float* buf, size_t n, float scale, int bf16, int grid) {
-  std::vector<std::function<void()>> bodies(1);
-  bodies[0] = bf16 ? std::function<void()>([=] { k0_cast_scale_kernel<true>(buf, n, scale); })
-                   : std::function<void()>([=] { k0_cast_scale_kernel<false>(buf, n, scale); });
-  return launch_all(1, grid, kThreads, bodies);
+  return launch_one(select_k0(bf16), grid, kThreads, buf, n, scale);
 }
 
 // Fused sharded step.  params live in every arena at `param_off`; grads[r], m[r], v[r] are plain buffers.
@@ -405,7 +356,7 @@ int emu_sharded_step64(void* h, int bf16, float** grads, size_t param_off, float
   const size_t half = (n * (bf16 ? 2 : 4) + 255) / 256 * 256;
   const size_t stage_base = param_off + ((n * 4 + 255) / 256 * 256);
   if (stage_base + 2 * half > g->arena_bytes) return -4;
-  std::vector<ShParams> params(world);
+  const auto kernel = select_k456(use_generic_w ? 0 : world, bf16);
   std::vector<std::function<void()>> bodies(world);
   for (int r = 0; r < world; ++r) {
     ShParams P{};
@@ -414,17 +365,11 @@ int emu_sharded_step64(void* h, int bf16, float** grads, size_t param_off, float
     P.exp_avg = m[r]; P.exp_avg_sq = v[r]; P.rs_out = nullptr; P.n = n;
     for (int i = 0; i <= world; ++i) P.off[i] = shard_off[i];
     for (int i = world + 1; i <= B2D_MAX_WORLD; ++i) P.off[i] = shard_off[world];
-    P.stage_off = stage_base + (parity & 1) * half; P.scale = scale; P.rank = r; P.world = world;
+    P.stage_off = stage_base + (parity & 1) * half; P.scale = scale;
     P.do_stage_reduce = 1; P.do_adam = 1; P.do_gather = 1; P.end_barrier = 0;
     P.adam = adam_consts(b2d_adam64{lr, beta1, beta2, eps, wd, step, adamw, 0, 0});
-    P.timeout_ns = 60ull * 1000000000ull; P.diag = nullptr; P.peers = make_peers(*g);
-    params[r] = P;
-    const ShParams* pp = &params[r];
-    dispatch_world(use_generic_w ? 0 : world, [&](auto w) {
-      constexpr int W = decltype(w)::value;
-      bodies[r] = bf16 ? std::function<void()>([=] { k456_sharded_kernel<W, true>(*pp); })
-                       : std::function<void()>([=] { k456_sharded_kernel<W, false>(*pp); });
-    });
+    set_peer_wait(&P, r, *g, 60);
+    bodies[r] = [=] { kernel(P); };
   }
   return launch_all(world, grid, kThreads, bodies);
 }
@@ -443,20 +388,17 @@ int emu_reduce_scatter(void* h, int bf16, float** grads, float** outs, size_t n,
   const int world = g->world;
   const size_t half = (n * (bf16 ? 2 : 4) + 255) / 256 * 256;
   if (stage_base + 2 * half > g->arena_bytes) return -4;
-  std::vector<ShParams> params(world);
+  const auto kernel = select_k456(0, bf16);
   std::vector<std::function<void()>> bodies(world);
   for (int r = 0; r < world; ++r) {
     ShParams P{};
     P.grads = grads[r]; P.rs_out = outs[r]; P.n = n;
     for (int i = 0; i <= world; ++i) P.off[i] = shard_off[i];
     for (int i = world + 1; i <= B2D_MAX_WORLD; ++i) P.off[i] = shard_off[world];
-    P.stage_off = stage_base + (parity & 1) * half; P.scale = scale; P.rank = r; P.world = world;
+    P.stage_off = stage_base + (parity & 1) * half; P.scale = scale;
     P.do_stage_reduce = 1; P.do_adam = 0; P.do_gather = 0;
-    P.timeout_ns = 60ull * 1000000000ull; P.peers = make_peers(*g);
-    params[r] = P;
-    const ShParams* pp = &params[r];
-    bodies[r] = bf16 ? std::function<void()>([=] { k456_sharded_kernel<0, true>(*pp); })
-                     : std::function<void()>([=] { k456_sharded_kernel<0, false>(*pp); });
+    set_peer_wait(&P, r, *g, 60);
+    bodies[r] = [=] { kernel(P); };
   }
   return launch_all(world, grid, kThreads, bodies);
 }
@@ -464,18 +406,16 @@ int emu_reduce_scatter(void* h, int bf16, float** grads, float** outs, size_t n,
 int emu_allgather(void* h, size_t buf_off, size_t n, const long long* shard_off, int grid) {
   Group* g = static_cast<Group*>(h);
   const int world = g->world;
-  std::vector<ShParams> params(world);
+  const auto kernel = select_k456(0, false);
   std::vector<std::function<void()>> bodies(world);
   for (int r = 0; r < world; ++r) {
     ShParams P{};
     P.params = reinterpret_cast<float*>(g->arena[r] + buf_off); P.param_off = buf_off; P.n = n;
     for (int i = 0; i <= world; ++i) P.off[i] = shard_off[i];
     for (int i = world + 1; i <= B2D_MAX_WORLD; ++i) P.off[i] = shard_off[world];
-    P.rank = r; P.world = world; P.do_gather = 1; P.end_barrier = 1;
-    P.timeout_ns = 60ull * 1000000000ull; P.peers = make_peers(*g);
-    params[r] = P;
-    const ShParams* pp = &params[r];
-    bodies[r] = std::function<void()>([=] { k456_sharded_kernel<0, false>(*pp); });
+    P.do_gather = 1; P.end_barrier = 1;
+    set_peer_wait(&P, r, *g, 60);
+    bodies[r] = [=] { kernel(P); };
   }
   return launch_all(world, grid, kThreads, bodies);
 }
@@ -495,7 +435,7 @@ int emu_owner_table(const long long* segs, int nseg, int world, int bf16, long l
 
 // K15 + K16 (fwd = 1) or K15 + K17 (fwd = 0) of one BN exchange: rank r pushes (a[r], b[r], counts[r]) into the
 // region at region_off of every arena (a[r] / b[r] may be NULL: a zero row), then combines into out_a[r], out_b[r],
-// counts_out[r] and, when rm / rv are given, rank r's running statistics.  order as in emu_staged_allreduce (0 / 1).
+// counts_out[r] and, when rm / rv are given, rank r's running statistics.  order as in run_phases (0 / 1).
 int emu_bn_exchange(void* h, int fwd, int channels, const float** a, const float** b, const float* counts, float eps, float momentum,
                     float** out_a, float** out_b, int32_t** counts_out, float** rm, float** rv, size_t region_off, unsigned epoch,
                     int grid, int order) {
@@ -503,37 +443,27 @@ int emu_bn_exchange(void* h, int fwd, int channels, const float** a, const float
   const int world = g->world;
   const size_t row = fwd ? bn_fwd_row(channels) : bn_bwd_row(channels);
   if (region_off + static_cast<size_t>(world) * row * 4 > g->arena_bytes) return -4;
-  const Peers peers = make_peers(*g);
-  auto push = [&](int r) {
+  auto push = [&](int r, int) {
     BnPushParams P{};
     P.a = a[r]; P.b = b[r]; P.count = fwd ? counts[r] : 0.f; P.channels = channels; P.fwd = fwd;
-    P.region_off = region_off; P.rank = r; P.world = world; P.epoch = epoch; P.peers = peers;
-    return launch_one(1, kBnThreads, [P] { bn_push_kernel(P); });
+    P.region_off = region_off; P.rank = r; P.world = world; P.epoch = epoch; P.peers = make_peers(*g);
+    return launch_one(bn_push_kernel, 1, kBnThreads, P);
   };
-  auto combine = [&](int r) {
+  auto combine = [&](int r, int) {
     BnCombineParams P{};
     P.region_off = region_off; P.channels = channels; P.eps = eps; P.momentum = momentum;
     P.out_a = out_a[r]; P.out_b = out_b[r]; P.counts = fwd ? counts_out[r] : nullptr;
     P.running_mean = rm ? rm[r] : nullptr; P.running_var = rv ? rv[r] : nullptr;
-    P.rank = r; P.world = world; P.epoch = epoch; P.timeout_ns = 120ull * 1000000000ull; P.diag = nullptr; P.peers = peers;
-    return fwd ? launch_one(grid, kBnThreads, [P] { bn_combine_kernel<true>(P); })
-               : launch_one(grid, kBnThreads, [P] { bn_combine_kernel<false>(P); });
+    P.epoch = epoch;
+    set_peer_wait(&P, r, *g, 120);
+    return launch_one(select_bn_combine(fwd), grid, kBnThreads, P);
   };
-  if (order == 1) {
-    for (int r = 0; r < world; ++r) if (push(r) != 0) return -1;
-    for (int r = 0; r < world; ++r) if (combine(r) != 0) return -1;
-    return 0;
-  }
-  std::atomic<int> bad{0};
-  std::vector<std::thread> streams;
-  for (int r = 0; r < world; ++r) streams.emplace_back([&, r] { if (push(r) != 0 || combine(r) != 0) bad = 1; });
-  for (auto& t : streams) t.join();
-  return bad.load() ? -1 : 0;
+  return run_phases(world, 1, order, {push, combine});
 }
 
 // K18 + K19 of one clip call, laid out as b2d.cu lays out the clip region at clip_off: [gen 0 | gen 1 | block sums].
 // x[r]: rank r's n[r] elements; norm_out[r] / coef_out[r]: one float each.  gmax: the block cap (kClipGMax in the
-// library).  order as in emu_staged_allreduce (0 / 1).
+// library).  order as in run_phases (0 / 1).
 int emu_clip_norm(void* h, const float** x, const size_t* n, float max_norm, float** norm_out, float** coef_out, size_t clip_off,
                   int gen, unsigned gmax, unsigned epoch, int order) {
   Group* g = static_cast<Group*>(h);
@@ -541,30 +471,21 @@ int emu_clip_norm(void* h, const float** x, const size_t* n, float max_norm, flo
   const size_t gen_bytes = static_cast<size_t>(world) * kClipSlotBytes;
   if (gmax < 1 || gmax > static_cast<unsigned>(kClipThreads)) return -2;
   if (clip_off + 2 * gen_bytes + gmax * sizeof(double) > g->arena_bytes) return -4;
-  const Peers peers = make_peers(*g);
-  auto partial = [&](int r) {
+  auto partial = [&](int r, int) {
     ClipPartialParams P{};
     P.x = x[r]; P.n = n[r]; P.vec = (reinterpret_cast<uintptr_t>(x[r]) % 16) == 0;
     P.block_sums = reinterpret_cast<double*>(g->arena[r] + clip_off + 2 * gen_bytes);
-    P.region_off = clip_off + (gen & 1) * gen_bytes; P.rank = r; P.world = world; P.epoch = epoch; P.peers = peers;
-    return launch_one(static_cast<int>(clip_grid(n[r], gmax)), kClipThreads, [P] { sqnorm_partial_kernel(P); });
+    P.region_off = clip_off + (gen & 1) * gen_bytes; P.rank = r; P.world = world; P.epoch = epoch; P.peers = make_peers(*g);
+    return launch_one(sqnorm_partial_kernel, static_cast<int>(clip_grid(n[r], gmax)), kClipThreads, P);
   };
-  auto coef = [&](int r) {
+  auto coef = [&](int r, int) {
     ClipCoefParams P{};
     P.region_off = clip_off + (gen & 1) * gen_bytes; P.max_norm = max_norm; P.norm_out = norm_out[r]; P.coef_out = coef_out[r];
-    P.rank = r; P.world = world; P.epoch = epoch; P.timeout_ns = 120ull * 1000000000ull; P.diag = nullptr; P.peers = peers;
-    return launch_one(1, 32, [P] { clip_coef_kernel(P); });
+    P.epoch = epoch;
+    set_peer_wait(&P, r, *g, 120);
+    return launch_one(clip_coef_kernel, 1, 32, P);
   };
-  if (order == 1) {
-    for (int r = 0; r < world; ++r) if (partial(r) != 0) return -1;
-    for (int r = 0; r < world; ++r) if (coef(r) != 0) return -1;
-    return 0;
-  }
-  std::atomic<int> bad{0};
-  std::vector<std::thread> streams;
-  for (int r = 0; r < world; ++r) streams.emplace_back([&, r] { if (partial(r) != 0 || coef(r) != 0) bad = 1; });
-  for (auto& t : streams) t.join();
-  return bad.load() ? -1 : 0;
+  return run_phases(world, 1, order, {partial, coef});
 }
 
 unsigned emu_clip_gmax(void) { return kClipGMax; }
