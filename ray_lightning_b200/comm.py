@@ -24,6 +24,7 @@ import torch.distributed as dist
 
 from . import _b2d
 from ._b2d import ALGO_NAMES, FLAG_MEM_VMM, FLAG_TIMING, WIRE_NAMES, AdamParams, B2DError
+from ._optim import kernel_args
 
 __all__ = ["Communicator", "LoopbackGroup", "B200HookState", "b200_allreduce_hook", "arena_bytes_for",
            "arena_tensor", "ArenaBufferSync", "b200_buffer_hook", "InBackwardOptimizer"]
@@ -605,16 +606,8 @@ class InBackwardOptimizer(torch.optim.Optimizer):
         if len(base.param_groups) != 1:
             raise ValueError("optimizer-in-backward supports one parameter group")
         g = base.param_groups[0]
-        if isinstance(base, torch.optim.SGD):
-            if g.get("nesterov") or g.get("dampening", 0) != 0 or g.get("maximize"):
-                raise ValueError("optimizer-in-backward SGD: no nesterov / dampening / maximize")
-            self.kind = 0
-        elif type(base) in (torch.optim.Adam, torch.optim.AdamW):
-            if g.get("amsgrad") or g.get("maximize") or g.get("capturable") or isinstance(g.get("lr"), torch.Tensor):
-                raise ValueError("optimizer-in-backward Adam: no amsgrad / maximize / capturable / tensor lr")
-            self.kind = 1
-        else:
-            raise ValueError("optimizer-in-backward supports SGD, Adam and AdamW (got %s)" % type(base).__name__)
+        kernel_args(type(base), base.defaults, g)      # NotFusable (a ValueError) names what K14 does not implement
+        self.kind = 0 if type(base) is torch.optim.SGD else 1
         self._base_cls = type(base)
         d = {k: v for k, v in g.items() if k != "params"}
         d["params"] = list(g["params"])
@@ -657,17 +650,10 @@ class InBackwardOptimizer(torch.optim.Optimizer):
                                     None if st[0][1] is None else [s[1].data_ptr() for s in st],
                                     offs, [p.numel() for p in params])
             self._tables[idx] = sig
-        g = self.param_groups[0]
-        if self.kind == 0:
-            hp = AdamParams(lr=float(g["lr"]), beta1=0.0, beta2=0.0, eps=0.0, weight_decay=float(g.get("weight_decay", 0.0)),
-                            step=self._steps + 1, adamw=0, zero_grads=0)
-            mom = float(g.get("momentum", 0.0))
-        else:
-            hp = AdamParams(lr=float(g["lr"]), beta1=float(g["betas"][0]), beta2=float(g["betas"][1]), eps=float(g["eps"]),
-                            weight_decay=float(g["weight_decay"]), step=self._steps + 1,
-                            adamw=int(self._base_cls is torch.optim.AdamW), zero_grads=0)
-            mom = 0.0
-        comm.ctx.bucket_optim(idx, buf.data_ptr(), buf.numel(), self.kind, hp, mom, stream)
+        a = kernel_args(self._base_cls, self.defaults, self.param_groups[0])
+        hp = AdamParams(lr=a["lr"], beta1=a.get("beta1", 0.0), beta2=a.get("beta2", 0.0), eps=a.get("eps", 0.0),
+                        weight_decay=a["weight_decay"], step=self._steps + 1, adamw=a.get("adamw", 0), zero_grads=0)
+        comm.ctx.bucket_optim(idx, buf.data_ptr(), buf.numel(), self.kind, hp, a.get("momentum", 0.0), stream)
         self.applied += 1
 
     @torch.no_grad()

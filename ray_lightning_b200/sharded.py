@@ -26,6 +26,7 @@ from typing import List
 
 import torch
 
+from ._optim import NotFusable, kernel_args
 from .partition import flat_layout, partition_parameters
 
 
@@ -90,16 +91,15 @@ class FlatShards:
                 p.grad = self.flat_grads[off:off + n].view(p.shape)
 
 
-_FUSABLE = (torch.optim.Adam, torch.optim.AdamW)
-
-
 def _fusable(opt: torch.optim.Optimizer) -> bool:
-    if type(opt) not in _FUSABLE or len(opt.param_groups) > 8:
+    """K13 steps Adam / AdamW with up to 8 parameter groups, each of a configuration kernel_args() accepts."""
+    if type(opt) not in (torch.optim.Adam, torch.optim.AdamW) or len(opt.param_groups) > 8:
         return False
-    for g in opt.param_groups:
-        if (g.get("amsgrad") or g.get("maximize") or g.get("capturable") or g.get("differentiable")
-                or isinstance(g.get("lr"), torch.Tensor)):
-            return False
+    try:
+        for g in opt.param_groups:
+            kernel_args(type(opt), opt.defaults, g)
+    except NotFusable:
+        return False
     return True
 
 
@@ -293,13 +293,14 @@ class ShardedOptimizer(torch.optim.Optimizer):
         cur, side = self._streams()
         self._flush()                  # staging zeroes the gradients it ships: after this the flat buffer is clean
         self._grads_clean = True
+        if side is not None and side is not cur:
+            side.wait_stream(cur)      # the step rewrites parameters and state that work queued before it may still read
+
         if self.fused:
             groups = []
             for g, (lo, hi) in zip(self.param_groups, self.group_range):
                 if hi > lo:
-                    groups.append((lo, hi, dict(lr=float(g["lr"]), beta1=float(g["betas"][0]), beta2=float(g["betas"][1]),
-                                                eps=float(g["eps"]), weight_decay=float(g["weight_decay"]),
-                                                step=self._steps, adamw=int(self._base_cls is torch.optim.AdamW))))
+                    groups.append((lo, hi, dict(kernel_args(self._base_cls, self.defaults, g), step=self._steps)))
             clip = {} if self._coef is None else {"grad_scale": self._coef}
             self.comm.adam_push_(sh.flat_params, self.exp_avg, self.exp_avg_sq, sh.reduced, sh.shard_off, groups,
                                  nvls=self.nvls, wait_stream=side, comm_stream=side, **clip)

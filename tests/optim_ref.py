@@ -216,6 +216,28 @@ def sgd_step64(p, g, buf, *, lr, momentum=0.0, weight_decay=0.0):
     return p, buf
 
 
+def sgd_bound64(p, g, buf, *, lr, momentum=0.0, weight_decay=0.0):
+    """The error an fp32 SGD step may carry against sgd_step64, for (p, buf): a few roundings of 2^-24 times the
+    magnitudes of the terms of each update (the decayed gradient, the momentum buffer, the parameter), plus a
+    subnormal-sized floor.  An fp32 implementation of torch's order of operations stays inside whether or not it
+    contracts `a + b * c` into a fused multiply-add (torch's single-tensor, foreach and fused kernels differ there).
+    `buf` is the buffer before the step (None on the first step with momentum); the buffer's bound is None without
+    momentum."""
+    e, floor = 2.0 ** -24, 2.0 ** -148
+    p, g = np.asarray(p, f32).astype(f64), np.asarray(g, f32).astype(f64)
+    with np.errstate(invalid="ignore", over="ignore"):
+        gmag = np.abs(g) + np.abs(weight_decay * p)
+        tol_g = 2 * e * gmag + floor
+        tol_b = None
+        if momentum != 0:
+            bmag = gmag if buf is None else momentum * np.abs(np.asarray(buf, f32).astype(f64)) + gmag
+            tol_b = tol_g + 3 * e * bmag + floor
+            tol_g, gmag = tol_b, bmag
+        pn, _ = sgd_step64(p.astype(f32), g.astype(f32), buf, lr=lr, momentum=momentum, weight_decay=weight_decay)
+        tol_p = lr * tol_g + 2 * e * (np.abs(p) + lr * gmag + np.abs(pn)) + floor
+    return tol_p, tol_b
+
+
 # ---- the grid the tests run ------------------------------------------------------------------------------------------
 BETAS = [(0.9, 0.999), (0.9, 0.95), (0.0, 0.99), (0.5, 0.9), (0.3, 0.999)]
 EPS = [1e-8, 1e-6, 1e-12]
